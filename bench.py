@@ -31,7 +31,7 @@ WORKLOADS = {
     "conformer_large_joint_32x15s": (dict(d_model=512, heads=8, ff=2048, enc_layers=12, dec_layers=6, vocab=5000, kernel=31), 15, 32, 10, 0.3, -64.0),
     "conformer_4l256_joint_8x5s": (dict(d_model=256, heads=4, ff=2048, enc_layers=4, dec_layers=2, vocab=5000, kernel=31), 5, 8, 10, 0.3, -16.0),
     # next scope row (SURVEY.md 8f-1 / BASELINE configs[4]): Transformer 24L/1024d/16h enc + 6L dec, attention-only beam 5; 64 utterances per GPU
-    # keep the conv1 planes within HBM (measured line: profiles/r02_bench_transformer_24l1024_att_64x30s_n1.json).
+    # keep the conv1 planes within the 80 GB of an H100.
     "transformer_24l1024_att_64x30s": (dict(d_model=1024, heads=16, ff=4096, enc_layers=24, dec_layers=6, vocab=5000, encoder="transformer"),
                                        30, 64, 5, 0.0, -64.0),
 }
@@ -39,7 +39,7 @@ WORKLOADS = {
 # lm 0.6 with a Transformer LM): the same Conformer-large + the Librispeech LM shape (16L / 512d / 8h / 2048 units, embed 128), 16 utterances per GPU.
 WORKLOADS["conformer_large_lm_beam60_16x30s"] = (WORKLOADS["conformer_large_joint_64x30s"][0], 30, 16, 60, 0.3, -64.0)
 LM_FUSION = {"conformer_large_lm_beam60_16x30s": dict(weight=0.6, conf=dict(pos_enc="sinusoidal", embed_unit=128, att_unit=512, head=8, unit=2048, layer=16))}
-METRIC = "utterances/sec (RTF) Conformer-large ASR inference at 1/2/4/8 B200 vs CPU ref"
+METRIC = "utterances/sec (RTF) Conformer-large ASR inference at 1/2/4/8 H100 vs CPU ref"
 # BASELINE.json configs[3] (next row 8f-2): contextual-block Conformer (12L/512d/8h, block 40 / hop 16 / look-ahead 16), 128 live streams per GPU,
 # 40-ms pushes (640 samples).  One "step" = 64 pushes (2.56 s of audio per stream); value = audio seconds processed per second (all streams).
 STREAMING = {"streaming_cbconformer_128x40ms": dict(streams=128, push=640, pushes_per_step=64, d_model=512, heads=8, ff=2048, layers=12, vocab=5000)}
@@ -90,9 +90,8 @@ REF_THREADS = 8
 
 
 def ref_workers():
-    """Decoding processes of the CPU arm.  Default 1: the reference decodes batch-1 in one process, and one 30-s utterance takes ~13 s on 8 threads,
-    which lets the arm honour the driver's --steps within a few minutes.  ESPB_REF_WORKERS=8 (8 x 8 threads) was measured on the 128-thread GPU host:
-    51 s per step of 8 utterances = 0.156 utt/s, i.e. 2x the single process -- the processes slow each other down 4x."""
+    """Decoding processes of the CPU arm.  Default 1: the reference decodes batch-1 in one process, so that the arm honours --steps within a few
+    minutes; ESPB_REF_WORKERS=n runs n processes of 8 threads each."""
     return int(os.environ.get("ESPB_REF_WORKERS", 1))
 
 
@@ -200,7 +199,7 @@ def ref_sample_desc(secs, mlr, workers, beam, workload=None):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -246,13 +245,90 @@ class ClockSampler:
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx, "samples": len(sm), "reasons": sorted(reasons)}
 
 
-def measured_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            d = json.load(f)
-        return d.get("bf16_tflops_sustained", 1400.0), d.get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json, bf16 sustained)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+def datasheet_peaks():
+    """Dense BF16 TFLOP/s and HBM3 GB/s of the H100 SXM data sheet (a card allowed 700 W; a lower power limit lowers the clocks)."""
+    return 989.0, 3350.0, "H100 SXM data sheet (dense BF16, HBM3), not measured"
+
+
+def gpu_identity(index):
+    """Name and power limit of the card the numbers were measured on (read-only nvidia-smi query)."""
+    out = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=30)
+        out["power_limit_w"] = float(r.stdout.strip().splitlines()[0])
+    except Exception:
+        pass
+    return out
+
+
+def dump_outputs(directory, arrays):
+    """Write {name: array} as directory/<name>.npy (float32 / float64): what the timed path returned in its last step."""
+    import numpy as np
+
+    os.makedirs(directory, exist_ok=True)
+    total = 0
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        a = a.astype(np.float64 if a.dtype == np.float64 or a.dtype.kind in "iu" else np.float32)
+        total += a.nbytes
+        np.save(os.path.join(directory, name + ".npy"), a)
+    assert total <= 64 * 1024 * 1024, f"dumped outputs are {total} bytes (> 64 MiB)"
+
+
+def gather_arrays(arrays, world):
+    """With several ranks: every rank's {name: array} (its utterance shard) concatenated along axis 0 in rank order, 2-D arrays padded with -1 to
+    the widest shard.  A collective: every rank calls it."""
+    if world == 1:
+        return arrays
+    import numpy as np
+    import torch.distributed as dist
+
+    shards = [None] * world
+    dist.all_gather_object(shards, {k: np.asarray(v) for k, v in arrays.items()})
+    out = {}
+    for k in arrays:
+        parts = [sh[k] for sh in shards]
+        if parts[0].ndim == 2:
+            width = max(p.shape[1] for p in parts)
+            parts = [np.pad(p, ((0, 0), (0, width - p.shape[1])), constant_values=-1.0) for p in parts]
+        out[k] = np.concatenate(parts, axis=0)
+    return out
+
+
+def tokens_arrays(toks):
+    """Per-stream token lists -> padded token ids (-1) and lengths (float64)."""
+    import numpy as np
+
+    L = max([len(t) for t in toks] + [0])
+    arr = np.full((len(toks), L), -1.0)
+    for i, t in enumerate(toks):
+        arr[i, :len(t)] = [int(x) for x in t]
+    return {"tokens": arr, "lengths": np.array([len(t) for t in toks], dtype=np.float64)}
+
+
+def hyps_arrays(res):
+    """BatchBeamSearch.forward_batch result (per utterance: n-best Hypothesis list) -> best hypothesis per utterance -> padded token ids (-1), lengths, total score and per-scorer scores (float64)."""
+    import numpy as np
+
+    best = [r[0] if r else None for r in res]
+    L = max([len(h.yseq) for h in best if h is not None] + [0])
+    tokens = np.full((len(best), L), -1.0)
+    lengths, score = np.zeros(len(best)), np.full(len(best), np.nan)
+    names = sorted({k for h in best if h is not None for k in h.scores})
+    per = {k: np.full(len(best), np.nan) for k in names}
+    for i, h in enumerate(best):
+        if h is None:
+            continue
+        y = h.yseq.tolist() if torch.is_tensor(h.yseq) else list(h.yseq)
+        tokens[i, :len(y)] = y
+        lengths[i], score[i] = len(y), float(h.score)
+        for k in names:
+            if k in h.scores:
+                per[k][i] = float(h.scores[k])
+    out = {"tokens": tokens, "lengths": lengths, "score": score}
+    out.update({"score_" + k: v for k, v in per.items()})
+    return out
 
 
 # ----------------------------------------------------------------------------------------------- reference arm (CPU)
@@ -304,37 +380,6 @@ def run_reference(args, rank, world):
 
 
 # ----------------------------------------------------------------------------------------------- espnet_b200 arm
-# DRAM traffic of ONE launch of the dominant kernel, from the committed `ncu --set full` capture (scripts/gpu_ncu_micro.sh ffn 2cta):
-# the encoder feed-forward w_1 GEMM of this workload (M 59968, N 2048, K 512, Swish, hi/lo split output).  dram__bytes_read.sum +
-# dram__bytes_write.sum; the algorithmic bytes are the hi/lo A and B planes read once and the hi/lo C planes written once.
-NCU_TRAFFIC = {"launch": "gemm_tf32x3_2cta_kernel<256,3,swish,split> M59968 N2048 K512", "dram_bytes": 275.803136e6 + 959.088128e6,
-               "algorithmic_bytes": (2 * 59968 * 512 + 2 * 2048 * 512 + 2 * 59968 * 2048) * 4.0, "gpu_time_us_under_ncu": 627.264,
-               "tensor_pipe_active_pct": 61.13, "source": "profiles/r01_ncu_gemm_2cta_ffn_w1_summary.txt"}
-
-
-def _load_ncu_traffic():
-    """Prefer the round-2 capture of the same launch (16-warp epilogue) when its summary is committed: profiles/r02_ncu_gemm_2cta_ffn_w1_ew16_summary.txt,
-    written by scripts/ncu_summary.py from `ncu --set full` of scripts/gemm_enc_microbench.py (scripts/gpu_final.sh)."""
-    path = os.path.join(ROOT, "profiles", "r02_ncu_gemm_2cta_ffn_w1_ew16_summary.txt")
-    if not os.path.exists(path):
-        return
-    vals = {}
-    with open(path) as f:
-        for ln in f:
-            parts = ln.split()
-            if len(parts) >= 3 and parts[0] in ("gpu__time_duration.sum", "dram__bytes_read.sum", "dram__bytes_write.sum",
-                                                "sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_active"):
-                scale = {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0, "us": 1.0, "ms": 1e3, "ns": 1e-3, "%": 1.0}.get(parts[2], 1.0)
-                vals.setdefault(parts[0], float(parts[1].replace(",", "")) * scale)
-    if len(vals) == 4:
-        NCU_TRAFFIC.update(dram_bytes=vals["dram__bytes_read.sum"] + vals["dram__bytes_write.sum"], gpu_time_us_under_ncu=vals["gpu__time_duration.sum"],
-                           tensor_pipe_active_pct=vals["sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_active"],
-                           source="profiles/r02_ncu_gemm_2cta_ffn_w1_ew16_summary.txt")
-
-
-_load_ncu_traffic()
-
-
 def run_streaming(args, rank, local_rank, world):
     """Streaming workload: frontend chunking -> ContextualBlockConformerEncoder.forward_infer -> CTC greedy, N streams in lock step."""
     import argparse as _ap
@@ -358,11 +403,12 @@ def run_streaming(args, rank, local_rank, world):
     host = waveforms(w["streams"], w["push"] * w["pushes_per_step"], offset=rank * w["streams"]).pin_memory()
 
     def step():
-        n_tok = 0
+        toks = [[] for _ in range(w["streams"])]
         for p in range(w["pushes_per_step"]):
             new = s2t(host[:, p * w["push"]:(p + 1) * w["push"]], is_final=False)     # pinned host chunk -> device inside the call
-            n_tok += sum(len(t) for t in new)
-        return n_tok
+            for i, t in enumerate(new):
+                toks[i].extend(t)
+        return toks
 
     def barrier():
         if world > 1:
@@ -376,7 +422,7 @@ def run_streaming(args, rank, local_rank, world):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(args.steps):
-        step()
+        toks = step()
     e1.record()
     barrier()
     ms = e0.elapsed_time(e1)
@@ -385,6 +431,10 @@ def run_streaming(args, rank, local_rank, world):
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms = float(t[0])
+    if args.dump_outputs:   # CTC-greedy tokens each stream emitted during the last timed step, all ranks' streams
+        dumped = gather_arrays(tokens_arrays(toks), world)
+        if rank == 0:
+            dump_outputs(args.dump_outputs, dumped)
     if rank != 0:
         return
     audio_s = world * w["streams"] * w["pushes_per_step"] * args.steps * w["push"] / 16000.0
@@ -397,7 +447,7 @@ def run_streaming(args, rank, local_rank, world):
                        "model": "contextual-block Conformer 12L/512d/8h block 40 hop 16 look-ahead 16, V=5000, CTC greedy",
                        "note": "next-row workload (SURVEY 8f-2): host chunks are copied inside the timed region; no beam search"},
             "e2e": {"value": val, "unit": "audio-s/s", "h2d_bytes_per_step": w["streams"] * w["push"] * w["pushes_per_step"] * 4, "d2h_bytes_per_step": 0},
-            "gpu_launches": ops.launch_counter[0], "clocks": clocks}
+            "gpu_launches": ops.launch_counter[0], "clocks": clocks, "gpu": gpu_identity(local_rank)}
     print(json.dumps(line), flush=True)
 
 
@@ -423,7 +473,7 @@ def run_b200(args, rank, local_rank, world):
     s2t = speech2text(cfg, model_weights(cfg), beam_size=beam, ctc_weight=ctcw, maxlenratio=mlr, nbest=1, **kw)
     host = waveforms(batch, nsamp, offset=rank * batch).pin_memory()      # utterances sharded by rank
     lens = torch.full((batch,), nsamp, dtype=torch.long)
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 50 MB L2
 
     def barrier():
         if world > 1:
@@ -553,7 +603,7 @@ def run_b200(args, rank, local_rank, world):
     for a, b in ev:
         flush.zero_()
         a.record()
-        res = step_resident(speech_dev)
+        res_resident = step_resident(speech_dev)
         b.record()
     barrier()
     wall = time.perf_counter() - wall0
@@ -569,20 +619,20 @@ def run_b200(args, rank, local_rank, world):
     e2e_ms = e0.elapsed_time(e1)
     clocks = sampler.stop()
     n_hyp_tokens = sum(len(r[0][2]) for r in res if r)
+    if args.dump_outputs:   # all ranks' utterances, in rank (= utterance) order
+        dumped = gather_arrays(hyps_arrays(res_resident), world)
+        if rank == 0:
+            dump_outputs(args.dump_outputs, dumped)
 
-    # ---- roofline of the dominant kernel (tcgen05 3xTF32 GEMM): per-launch CUDA events over one extra step
+    # ---- roofline of the dominant kernel (wgmma 3xTF32 GEMM): per-launch CUDA events over one extra step
     ops.gemm_profile = []
     step_resident(speech_dev)
     torch.cuda.synchronize()
     prof = ops.gemm_profile
     ops.gemm_profile = None
-    big = [p for p in prof if p[3]]          # gemm_tf32x3_2cta_kernel launches (the dominant kernel)
-    small = [p for p in prof if not p[3]]    # gemm_tf32x3_kernel (1-CTA tiles, decode-step problems)
-    g_flops = sum(p[0] for p in big)
-    g_ms = sum(p[1].elapsed_time(p[2]) for p in big)
-    s_flops = sum(p[0] for p in small)
-    s_ms = sum(p[1].elapsed_time(p[2]) for p in small)
-    peak_tf, hbm_gbs, peak_src = measured_peaks()
+    g_flops = sum(p[0] for p in prof)
+    g_ms = sum(p[1].elapsed_time(p[2]) for p in prof)
+    peak_tf, hbm_gbs, peak_src = datasheet_peaks()
     # ---- the other kernels the north star names, timed live (CUDA events around every C-ABI call of one un-graphed step)
     from espnet_b200 import lib as _lib
 
@@ -642,7 +692,7 @@ def run_b200(args, rank, local_rank, world):
         "data": "synthetic", "rtf": (dev_ms / 1000.0) / (utts * secs),
         "config": {"workload": args.workload, "global_batch": world * batch, "utt_seconds": secs, "beam": beam, "ctc_weight": ctcw,
                    "maxlenratio": mlr, "vocab": cfg["vocab"], "parallelism": f"utterance-sharded x{world}", "l2": "flushed between steps (256 MiB write)",
-                   "gemm": "tcgen05 kind::tf32 x3 (error-compensated fp32), mode " + ops.gemm_mode(), "attention": ops.attn_mode(),
+                   "gemm": "wgmma tf32 x3 (error-compensated fp32), mode " + ops.gemm_mode(), "attention": ops.attn_mode(),
                    "wall_s_timed_region": wall,
                    **({"lm": {"type": "TransformerLM", "weight": LM_FUSION[args.workload]["weight"], **LM_FUSION[args.workload]["conf"]},
                        "decode_setup": "egs2/librispeech/asr1/conf/decode_asr.yaml:1-3 (beam 60, ctc 0.3, lm 0.6)"} if args.workload in LM_FUSION else {})},
@@ -652,13 +702,11 @@ def run_b200(args, rank, local_rank, world):
                 "hyp_tokens_last_step": n_hyp_tokens},
         "gpu_launches": launches,
         "clocks": clocks,
-        "roofline": {"bound": "tensor", "kernel": "gemm_tf32x3_2cta_kernel (all its launches in one step: encoder, CTC head, decoder memory)", "achieved": ach, "peak": peak_tf,
-                     "unit": "TFLOP/s", "frac": ach / peak_tf if peak_tf else None, "traffic": NCU_TRAFFIC["dram_bytes"], "traffic_launch": NCU_TRAFFIC,
-                     "peak_source": peak_src,
-                     "launches": len(big), "gemm_ms_per_step": g_ms, "algorithmic_tflop_per_step": g_flops / 1e12,
+        "gpu": gpu_identity(local_rank),
+        "roofline": {"bound": "tensor", "kernel": "gemm_tf32x3_kernel (all its launches in one un-graphed step)", "achieved": ach, "peak": peak_tf,
+                     "unit": "TFLOP/s", "frac": ach / peak_tf if peak_tf else None, "peak_source": peak_src,
+                     "launches": len(prof), "gemm_ms_per_step": g_ms, "algorithmic_tflop_per_step": g_flops / 1e12,
                      "frac_of_3xtf32_ceiling": (ach / (peak_tf / 6.0)) if peak_tf else None,
-                     "decode_gemm_1cta": {"kernel": "gemm_tf32x3_sk_kernel / gemm_tf32x3_mc_kernel / gemm_tf32x3_kernel (128-row 1-CTA tiles)", "launches": len(small), "ms_per_step_ungraphed": s_ms,
-                                          "achieved": (s_flops / (s_ms / 1000.0) / 1e12) if s_ms > 0 else None},
                      "note": "algorithmic FLOPs (2MNK); each is executed as 3 tf32 MMAs at half the bf16 rate, so 1/6 of the bf16 peak is the ceiling of this formulation",
                      "other_kernels": other},
     }
@@ -708,7 +756,13 @@ def main():
     ap.add_argument("--trace", action="store_true", help="CUPTI activity trace of one step (kernel durations inside the CUDA graphs) -> stderr")
     ap.add_argument("--breakdown", action="store_true", help="time every launch of one step with CUDA events and print a per-kernel table")
     ap.add_argument("--profile-one-step", action="store_true", help="warm up, then run one step inside cudaProfilerStart/Stop and exit")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last timed step of the CUDA path returned as "
+                    "DIR/<name>.npy (with several GPUs: every rank's utterances / streams, in rank order)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "b200":
+        ap.error("--dump-outputs records the CUDA path (--impl b200)")
+    if args.dump_outputs and args.steps < 1:
+        ap.error("--dump-outputs needs at least one timed step (--steps >= 1)")
     rank, local_rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("LOCAL_RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     if args.impl == "reference":
         run_reference(args, rank, world)

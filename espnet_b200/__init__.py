@@ -1,4 +1,4 @@
-"""espnet_b200: B200-native (sm_100a) implementation of ESPnet2's Speech2Text inference hot path.
+"""espnet_b200: H100-native (sm_90a) implementation of ESPnet2's Speech2Text inference hot path.
 
 Public surface mirrors the reference classes on that path (see SURVEY.md section 8b):
 Speech2Text, ESPnetASRModel, DefaultFrontend, UtteranceMVN, ConformerEncoder, CTC,

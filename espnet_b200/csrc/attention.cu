@@ -1,31 +1,21 @@
-// Fused self-attention of the encoders on the 5th-gen tensor cores: S = Q K^T (+ rel-pos term) -> masked online softmax -> O = P V in one
+// Fused self-attention of the encoders on the Hopper tensor cores: S = Q K^T (+ rel-pos term) -> masked online softmax -> O = P V in one
 // kernel; neither the scores nor the probabilities ever reach HBM.
 //
 // Reference semantics: RelPositionMultiHeadedAttention.forward / rel_shift / forward_attention
 // (espnet2/legacy/nets/pytorch_backend/transformer/attention.py:416-459, 391-414, 121-151) and, with bd == nullptr, the plain
 // MultiHeadedAttention.forward (:153-265): scores = (q_u k^T + bd[i][T-1-i+j]) / sqrt(d_k), keys j >= len masked, softmax, x = p v.
 //
-// Numerics: every product is an error-compensated 3xTF32 tcgen05 MMA (a_lo b_hi + a_hi b_lo + a_hi b_hi, fp32 accumulate) like the
-// GEMMs (gemm.cu).  The long accumulation over the keys does NOT run in the tensor core's truncating accumulator: every 64-key tile's
-// P V lands in a fresh TMEM buffer and is added into fp32 registers with round-to-nearest while the online-softmax rescale is applied.
+// Numerics: every product is an error-compensated 3xTF32 wgmma (a_lo b_hi + a_hi b_lo + a_hi b_hi, fp32 accumulate) like the GEMMs
+// (gemm.cu).  The long accumulation over the keys does NOT run in the tensor core: every 64-key tile's P V lands in a fresh wgmma
+// accumulator and is added into fp32 registers with round-to-nearest while the online-softmax rescale is applied.
 //
-// Work decomposition: one cluster of two CTAs (cta_group::2, UMMA M = 256) per (utterance, head, block of 256 queries); CTA r owns query
-// rows [256 qb + 128 r, +128) (one row per softmax thread = one TMEM lane) and stages its half of every B operand (32 of the 64 keys of
-// a K tile, 32 of the 64 d_k rows of a V^T tile), which halves the shared-memory fill and operand-read traffic per SM against a 1-CTA
-// kernel.  The A operands (Q hi/lo, P hi/lo) live in TENSOR MEMORY, so the MMAs read only the B tiles from shared memory.
-//
-//   warp 0 (lane 0)      TMA producer: K tiles, V^T tiles (SWIZZLE_128B, cta_group::2 loads signalling the leader's barriers) and, for
-//                        rel-pos attention, per softmax warp a 32 x 100 window of the UNSHIFTED bd = (q+v) p^T matrix (rel_shift is a
-//                        row-dependent column offset: row i needs bd[i][T-1-i+j]; TMA needs a 16-byte aligned start column, so the box
-//                        starts at the window start rounded down to a multiple of 4 -- the remainder T mod 4 is the same for every
-//                        window; an odd multiple of 4 floats as the unswizzled row pitch makes lane l's reads bank-conflict free)
-//   warp 1 (lane 0, leader CTA)  MMA issue: S(t) = Q K(t)^T into S[t&1] as soon as S(t-2) has been read; after P(t) is published:
-//                        O(t) = P(t) V(t) into O[t&1]
-//   warps 2-9            softmax, two warpgroups: thread = (query row, 32-column half).  S(t) from TMEM, + bd window from smem, scale, mask,
-//                        running max (exchanged between the halves through smem) / sum, P(t) hi/lo back to TMEM; O(t-1) from TMEM folded
-//                        into the fp32 register accumulator with the rescale factor.
-//
-// TMEM columns (512): Q hi 0-63 | Q lo 64-127 | S[0] 128-191 | S[1] 192-255 | P hi 256-319 | P lo 320-383 | O[0] 384-447 | O[1] 448-511.
+// Work decomposition: one CTA per (utterance, head, block of 128 queries), three warpgroups.
+//   warps 0-7  two consumer warpgroups; warpgroup g owns query rows [128 qb + 64 g, +64).  S = Q K^T with Q and K from shared memory,
+//              + rel-pos term bd[i][T-1-i+j] read from global memory (rel_shift is a row-dependent column offset of the unshifted
+//              bd = (q+v) p^T matrix), scale, mask, online softmax in registers; P hi/lo is rearranged from the accumulator layout into
+//              the register A-operand layout with quad shuffles, and O(t) = P(t) V(t) reads only V^T from shared memory.
+//   warp 8     TMA producer (one elected lane; its warpgroup hands its registers to the consumers): Q once, then K tiles and V^T tiles (SWIZZLE_128B, hi / lo planes) through a two-stage
+//              ring each; a consumer warpgroup releases a stage once its MMAs retired.
 #include <cuda.h>
 #include <math.h>
 #include <stdio.h>
@@ -38,332 +28,243 @@ namespace {
 
 using namespace espb::tc;
 
-#ifdef ESPB_ATTN_SLEEP_WAIT
-#define ATT_WAIT mbar_wait
-#else
-#define ATT_WAIT mbar_wait_spin
-#endif
-
 constexpr int DK = 64;                      // head dimension served by this kernel
 constexpr int KB = 64;                      // keys per tile
-constexpr int KV_STAGES = 3;
-constexpr int BD_STAGES = 2;
-constexpr int TILE_BYTES = 32 * 128;        // one [32 rows x 32 fp32] swizzled operand block
-constexpr int KV_STAGE_BYTES = 4 * TILE_BYTES;          // [hi | lo] x [k-block 0 | 1]
-constexpr int BD_COLS = 100;                 // 32 + 64 - 1 window columns + up to 3 columns of alignment slack, a multiple of 4
-constexpr int BD_WARP_BYTES = 32 * BD_COLS * 4;
-constexpr int BD_STAGE_BYTES = 4 * BD_WARP_BYTES;
-constexpr int ATT_THREADS = 320;                // warp 0: TMA, warp 1: MMA, warps 2-9: two softmax warpgroups
-constexpr uint32_t TM_QHI = 0, TM_QLO = 64, TM_S = 128, TM_PHI = 256, TM_PLO = 320, TM_O = 384;
+constexpr int QB = 128;                     // queries per CTA
+constexpr int KV_STAGES = 2;
+constexpr int BLK_BYTES = 64 * 128;         // one [64 rows x 32 fp32] swizzled operand block
+constexpr int Q_BYTES = 2 * 2 * 2 * BLK_BYTES;          // [hi | lo] x [d_k block 0 | 1] x [row block 0 | 1]
+constexpr int KV_STAGE_BYTES = 4 * BLK_BYTES;           // [hi | lo] x [k-block 0 | 1]
+constexpr int ATT_THREADS = 384;          // warpgroups 0-1: consumers, warpgroup 2: producer (one warp works)
 
 struct AttnParams {
   const float* q; long long q_plane, ldq;        // split Q-like tensor: element (row, c) of head h at q + row*ldq + h*DK + c (+ q_plane: lo)
   const int* lens;
+  const float* bd; int Rp;                       // unshifted rel-pos term [B][H][T][Rp] or null
   float* out; long long out_plane, ldo;          // split context [rows][H*DK]
-  int B, H, T, nqb;                              // nqb = ceil(T / 256)
+  int B, H, T, nqb;                              // nqb = ceil(T / 128)
   float scale;                                   // 1 / sqrt(d_k)
 };
 
 template <bool RELPOS>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(ATT_THREADS, 1)
-flash_attn_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmBD,
+__global__ void __launch_bounds__(ATT_THREADS, 1)
+flash_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                   AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t k_base = smem_base;
+  const uint32_t q_base = smem_base;
+  const uint32_t k_base = q_base + Q_BYTES;
   const uint32_t v_base = k_base + KV_STAGES * KV_STAGE_BYTES;
-  const uint32_t bd_base = v_base + KV_STAGES * KV_STAGE_BYTES;
-  const uint32_t bar_base = bd_base + (RELPOS ? BD_STAGES * BD_STAGE_BYTES : 0);
-  const uint32_t k_full = bar_base, k_empty = k_full + 8 * KV_STAGES, v_full = k_empty + 8 * KV_STAGES, v_empty = v_full + 8 * KV_STAGES;
-  const uint32_t bd_full = v_empty + 8 * KV_STAGES, bd_empty = bd_full + 8 * BD_STAGES;
-  const uint32_t s_full = bd_empty + 8 * BD_STAGES, o_full = s_full + 16, p_full = o_full + 16, q_full = p_full + 8, s_empty = q_full + 8;
-  uint8_t* smem_al = smem_raw + (smem_base - smem_u32(smem_raw));
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(smem_al + (s_empty + 16 - smem_base));
-  const uint32_t xch_base = s_empty + 32;        // row-maximum exchange between the two softmax warpgroups: [2][2][128] floats
+  const uint32_t bar_base = v_base + KV_STAGES * KV_STAGE_BYTES;
+  const uint32_t q_full = bar_base, k_full = q_full + 8, k_empty = k_full + 8 * KV_STAGES, v_full = k_empty + 8 * KV_STAGES,
+                 v_empty = v_full + 8 * KV_STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int item = blockIdx.x >> 1;
+  const int item = blockIdx.x;
   const int qb = item % p.nqb, h = (item / p.nqb) % p.H, b = item / (p.nqb * p.H);
   const int len = min(p.lens[b], p.T);
-  const int I0 = qb * 256;                     // first query row of the pair
-  const int R0 = I0 + (int)rank * 128;         // first query row of this CTA
+  const int I0 = qb * QB;                      // first query row of the CTA
   const int nkt = (len + KB - 1) / KB;
 
   if (I0 >= len || nkt == 0) {
-    // every query row of this pair is padding (t >= len): defined (zero) output, no tensor work.  Both CTAs take this branch together.
-    if (warp >= 2) {
-      const int row = R0 + (warp & 3) * 32 + lane;
+    // every query row of this block is padding (t >= len): defined (zero) output, no tensor work
+    for (int i = threadIdx.x; i < QB * (DK / 4); i += blockDim.x) {
+      const int row = I0 + i / (DK / 4), c = (i % (DK / 4)) * 4;
       if (row < p.T) {
-        float* o = p.out + ((long long)b * p.T + row) * p.ldo + h * DK + ((warp - 2) >> 2) * 32;
-        for (int c = 0; c < 32; c += 4) {
-          *reinterpret_cast<float4*>(o + c) = make_float4(0.f, 0.f, 0.f, 0.f);
-          *reinterpret_cast<float4*>(o + p.out_plane + c) = make_float4(0.f, 0.f, 0.f, 0.f);
-        }
+        float* o = p.out + ((long long)b * p.T + row) * p.ldo + h * DK + c;
+        *reinterpret_cast<float4*>(o) = make_float4(0.f, 0.f, 0.f, 0.f);
+        *reinterpret_cast<float4*>(o + p.out_plane) = make_float4(0.f, 0.f, 0.f, 0.f);
       }
     }
     return;
   }
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
+    mbar_init(q_full, 1);
     for (int s = 0; s < KV_STAGES; ++s) {
-      mbar_init(k_full + 8 * s, 1); mbar_init(k_empty + 8 * s, 1);
-      mbar_init(v_full + 8 * s, 1); mbar_init(v_empty + 8 * s, 1);
+      mbar_init(k_full + 8 * s, 1); mbar_init(k_empty + 8 * s, 2);   // empty: one arrival per consumer warpgroup
+      mbar_init(v_full + 8 * s, 1); mbar_init(v_empty + 8 * s, 2);
     }
-    for (int s = 0; s < BD_STAGES; ++s) { mbar_init(bd_full + 8 * s, 1); mbar_init(bd_empty + 8 * s, 8); }
-    for (int s = 0; s < 2; ++s) { mbar_init(s_full + 8 * s, 1); mbar_init(o_full + 8 * s, 1); }
-    mbar_init(p_full, 16);     // 8 softmax warps x 2 CTAs
-    mbar_init(q_full, 16);
-    mbar_init(s_empty, 16); mbar_init(s_empty + 8, 16);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmQ) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmK) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmV) : "memory");
-    if (RELPOS) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmBD) : "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  cluster_sync_all();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp == 0) {
-    // ===================================================================== TMA producer (one elected lane per CTA)
-    if (elect_one_sync()) {
+  if (warp >= 8) {
+    // ===================================================================== TMA producer (one elected lane)
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == 8 && elect_one_sync()) {
+      mbar_expect_tx(q_full, Q_BYTES);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {   // block i = (plane, d_k block, row block)
+        const int pl = i >> 2, kb = (i >> 1) & 1, rb = i & 1;
+        tma_load_5d(q_base + i * BLK_BYTES, &tmQ, q_full, kb * 32, I0 + rb * 64, h, b, pl);
+      }
       for (int t = 0; t < nkt; ++t) {
         const int s = t % KV_STAGES;
         const uint32_t ph = (uint32_t)((t / KV_STAGES) & 1);
         const int J0 = t * KB;
-        {  // K tile: this CTA's 32 keys x 64 d_k, hi/lo planes, two 32-wide k-blocks
-          ATT_WAIT(k_empty + 8 * s, ph ^ 1);
-          if (leader) mbar_expect_tx(k_full + 8 * s, 2 * KV_STAGE_BYTES);
-          const uint32_t fb = (k_full & 0xFEFFFFFFu) + 8 * s;       // the leader CTA's barrier
-          const uint32_t dst = k_base + s * KV_STAGE_BYTES;
-          const int row = J0 + (int)rank * 32;
-          tma_load_5d_2sm(dst, &tmK, fb, 0, row, h, b, 0);
-          tma_load_5d_2sm(dst + TILE_BYTES, &tmK, fb, 32, row, h, b, 0);
-          tma_load_5d_2sm(dst + 2 * TILE_BYTES, &tmK, fb, 0, row, h, b, 1);
-          tma_load_5d_2sm(dst + 3 * TILE_BYTES, &tmK, fb, 32, row, h, b, 1);
-        }
-        if (RELPOS) {  // bd windows: warp quarter q gets rows R0+32q.. and columns c0 = T-1-(row0+31)+J0 - (T&3) .. +99 (out-of-range -> zero fill)
-          const int sb = t % BD_STAGES;
-          ATT_WAIT(bd_empty + 8 * sb, (uint32_t)(((t / BD_STAGES) & 1) ^ 1));
-          mbar_expect_tx(bd_full + 8 * sb, BD_STAGE_BYTES);
-          for (int q = 0; q < 4; ++q) {
-            const int row0 = R0 + 32 * q;
-            tma_load_5d(bd_base + sb * BD_STAGE_BYTES + q * BD_WARP_BYTES, &tmBD, bd_full + 8 * sb, p.T - 1 - (row0 + 31) + J0 - (p.T & 3), row0, h, b, 0);
-          }
-        }
-        {  // V^T tile: this CTA's 32 d_k rows x 64 keys
-          ATT_WAIT(v_empty + 8 * s, ph ^ 1);
-          if (leader) mbar_expect_tx(v_full + 8 * s, 2 * KV_STAGE_BYTES);
-          const uint32_t fb = (v_full & 0xFEFFFFFFu) + 8 * s;
-          const uint32_t dst = v_base + s * KV_STAGE_BYTES;
-          const int drow = (int)rank * 32;
-          tma_load_5d_2sm(dst, &tmV, fb, J0, drow, h, b, 0);
-          tma_load_5d_2sm(dst + TILE_BYTES, &tmV, fb, J0 + 32, drow, h, b, 0);
-          tma_load_5d_2sm(dst + 2 * TILE_BYTES, &tmV, fb, J0, drow, h, b, 1);
-          tma_load_5d_2sm(dst + 3 * TILE_BYTES, &tmV, fb, J0 + 32, drow, h, b, 1);
-        }
+        mbar_wait(k_empty + 8 * s, ph ^ 1);
+        mbar_expect_tx(k_full + 8 * s, KV_STAGE_BYTES);
+#pragma unroll
+        for (int i = 0; i < 4; ++i)   // block i = (plane, d_k block): 64 keys x 32 d_k
+          tma_load_5d(k_base + s * KV_STAGE_BYTES + i * BLK_BYTES, &tmK, k_full + 8 * s, (i & 1) * 32, J0, h, b, i >> 1);
+        mbar_wait(v_empty + 8 * s, ph ^ 1);
+        mbar_expect_tx(v_full + 8 * s, KV_STAGE_BYTES);
+#pragma unroll
+        for (int i = 0; i < 4; ++i)   // block i = (plane, key block): 64 d_k rows x 32 keys of V^T
+          tma_load_5d(v_base + s * KV_STAGE_BYTES + i * BLK_BYTES, &tmV, v_full + 8 * s, J0 + (i & 1) * 32, 0, h, b, i >> 1);
       }
     }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer (leader CTA, one elected lane)
-    if (leader && elect_one_sync()) {
-      // D = f32, A = B = tf32, K-major, N = 64, M = 256 (cta_group::2)
-      const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-      auto issue_s = [&](int t) {
-        const int s = t % KV_STAGES;
-        ATT_WAIT(k_full + 8 * s, (uint32_t)((t / KV_STAGES) & 1));
-        tcgen05_fence_after();
-        const uint32_t kb_smem = k_base + s * KV_STAGE_BYTES;
-        const uint32_t d = tmem_base + TM_S + (uint32_t)(t & 1) * 64;
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {     // 8 tf32 per MMA: d_k = 64 -> 8 steps
-          const uint32_t off = (uint32_t)(kk >> 2) * TILE_BYTES + (uint32_t)(kk & 3) * 32;
-          const uint64_t b_hi = umma_desc(kb_smem + off), b_lo = umma_desc(kb_smem + 2 * TILE_BYTES + off);
-          const uint32_t a_hi = tmem_base + TM_QHI + kk * 8, a_lo = tmem_base + TM_QLO + kk * 8;
-          mma_tf32_2sm_ta(d, a_lo, b_hi, idesc, kk != 0);
-          mma_tf32_2sm_ta(d, a_hi, b_lo, idesc, 1);
-          mma_tf32_2sm_ta(d, a_hi, b_hi, idesc, 1);
-        }
-        tcgen05_commit_2sm(k_empty + 8 * s);
-        tcgen05_commit_2sm(s_full + 8 * (t & 1));
-      };
-      ATT_WAIT(q_full, 0);
-      tcgen05_fence_after();
-      issue_s(0);
-      if (nkt > 1) issue_s(1);
-      for (int t = 0; t < nkt; ++t) {
-        const int s = t % KV_STAGES;
-        if (t + 2 < nkt) {   // S(t) is in the softmax threads' registers: its buffer takes S(t+2), which then runs under softmax(t) instead of
-          ATT_WAIT(s_empty + 8 * (t & 1), (uint32_t)((t >> 1) & 1));   // queueing between P V(t) and P V(t+1) on the in-order tensor pipe
-          tcgen05_fence_after();
-          issue_s(t + 2);
-        }
-        ATT_WAIT(p_full, (uint32_t)(t & 1));        // P(t) is in TMEM in both CTAs; O(t-2) has been consumed
-        ATT_WAIT(v_full + 8 * s, (uint32_t)((t / KV_STAGES) & 1));
-        tcgen05_fence_after();
-        const uint32_t vb_smem = v_base + s * KV_STAGE_BYTES;
-        const uint32_t d = tmem_base + TM_O + (uint32_t)(t & 1) * 64;
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {     // 64 keys -> 8 steps
-          const uint32_t off = (uint32_t)(kk >> 2) * TILE_BYTES + (uint32_t)(kk & 3) * 32;
-          const uint64_t b_hi = umma_desc(vb_smem + off), b_lo = umma_desc(vb_smem + 2 * TILE_BYTES + off);
-          const uint32_t a_hi = tmem_base + TM_PHI + kk * 8, a_lo = tmem_base + TM_PLO + kk * 8;
-          mma_tf32_2sm_ta(d, a_lo, b_hi, idesc, kk != 0);
-          mma_tf32_2sm_ta(d, a_hi, b_lo, idesc, 1);
-          mma_tf32_2sm_ta(d, a_hi, b_hi, idesc, 1);
-        }
-        tcgen05_commit_2sm(v_empty + 8 * s);
-        tcgen05_commit_2sm(o_full + 8 * (t & 1));
-      }
-    }
-  } else {
-    // ===================================================================== softmax / accumulate: two warpgroups, thread = (query row, half)
-    // Warps w and w + 4 own the same TMEM lane quarter (rows); group g = 0 / 1 handles key columns [32g, 32g+32) of every S tile and
-    // output columns [32g, 32g+32) of O.  The two threads of a row agree on the running maximum through shared memory (one 64-thread
-    // named barrier per tile); their partial row sums are only combined at the end (same maxima -> the partial sums simply add).
-    const int q = warp & 3;                                   // TMEM lane quarter of this warp
-    const int g = (warp - 2) >> 2;                            // column half
-    const uint32_t tlane = ((uint32_t)(q * 32)) << 16;
-    const int rloc = q * 32 + lane;                           // row within the CTA
-    const int row = R0 + rloc;
-    const uint32_t cg = (uint32_t)g * 32;
-    float* xch = reinterpret_cast<float*>(smem_al + (xch_base - smem_base));    // [2 parities][2 groups][128 rows]
-    {  // Q hi/lo of this row, columns [32g, 32g+32) -> TMEM (rows >= T: zeros)
-      const float* qp = p.q + ((long long)b * p.T + row) * p.ldq + h * DK + cg;
-#pragma unroll
-      for (int pl = 0; pl < 2; ++pl) {
-        float v[32];
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (row < p.T) x = __ldg(reinterpret_cast<const float4*>(qp + pl * p.q_plane + j));
-          v[j] = x.x; v[j + 1] = x.y; v[j + 2] = x.z; v[j + 3] = x.w;
-        }
-        tmem_st32(tmem_base + tlane + (pl ? TM_QLO : TM_QHI) + cg, v);
-      }
-      tmem_st_wait();
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(q_full, 0);
-    }
-    float o_acc[32];
-#pragma unroll
-    for (int j = 0; j < 32; ++j) o_acc[j] = 0.f;
-    float m_run = -INFINITY, l_run = 0.f, alpha_prev = 0.f;
-    const float scale = p.scale;
-    // this lane's window of the bd tile: row `lane` of the quarter's [32][100] block, starting at column 31 - lane + (T & 3) + 32g
-    // (bank = (3 * lane + const + j) mod 32: distinct over the warp)
-    const float* bd_lane = reinterpret_cast<const float*>(smem_al + (bd_base - smem_base) + q * BD_WARP_BYTES) + lane * BD_COLS + (31 - lane) + (p.T & 3) + cg;
+    return;
+  }
 
-    for (int t = 0; t < nkt; ++t) {
-      const int J0 = t * KB + (int)cg;                        // first key of this thread's 32 columns
-      float s[32];
-      ATT_WAIT(s_full + 8 * (t & 1), (uint32_t)((t >> 1) & 1));
-      tcgen05_fence_after();
-      tmem_ld32_nowait(tmem_base + tlane + TM_S + (uint32_t)(t & 1) * 64 + cg, s);
-      tmem_ld_wait();
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(s_empty + 8 * (t & 1), 0);     // the S buffer may be overwritten (by S(t+2))
-      if (RELPOS) {
-        const int sb = t % BD_STAGES;
-        ATT_WAIT(bd_full + 8 * sb, (uint32_t)((t / BD_STAGES) & 1));
-        const float* a = bd_lane + sb * (BD_STAGE_BYTES / 4);
+  // ===================================================================== consumers: thread = (rows ra, ra + 8; 16 of the 64 columns)
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int g = warp >> 2;
+  const int ra = I0 + g * 64 + (warp & 3) * 16 + (lane >> 2), rb = ra + 8;
+  const int tq = lane & 3;
+  const int src0 = (lane & ~3) | (tq >> 1), src1 = src0 + 2;   // quad lanes holding P columns tq and tq + 4 of an 8-key group
+  const uint32_t qa = q_base + g * BLK_BYTES;                   // this warpgroup's 64 rows of Q
+  const float scale = p.scale;
+  const float* bd_a = nullptr;
+  const float* bd_b = nullptr;
+  if (RELPOS) {
+    const long long head = ((long long)b * p.H + h) * p.T;
+    if (ra < p.T) bd_a = p.bd + (head + ra) * p.Rp + (p.T - 1 - ra);
+    if (rb < p.T) bd_b = p.bd + (head + rb) * p.Rp + (p.T - 1 - rb);
+  }
+  float o_acc[32], ot[32], s[32];
 #pragma unroll
-        for (int j = 0; j < 32; ++j) s[j] += a[j];
-        __syncwarp();
-        if (lane == 0) mbar_arrive_local(bd_empty + 8 * sb);
-      }
-      if (J0 + 32 > len) {
+  for (int j = 0; j < 32; ++j) o_acc[j] = 0.f;
+  float m_a = -INFINITY, m_b = -INFINITY, l_a = 0.f, l_b = 0.f;
+  mbar_wait_spin(q_full, 0);
+
+  for (int t = 0; t < nkt; ++t) {
+    const int st = t % KV_STAGES;
+    const uint32_t ph = (uint32_t)((t / KV_STAGES) & 1);
+    const int J0 = t * KB;
+    // ---- S = Q K^T
+    mbar_wait_spin(k_full + 8 * st, ph);
+    const uint32_t kt = k_base + st * KV_STAGE_BYTES;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) if (J0 + j >= len) s[j] = -INFINITY;
-      }
-      float mt = s[0];
+    for (int j = 0; j < 32; ++j) s[j] = 0.f;   // the first MMA ignores the old value: keeps the previous tile's registers dead
+    fence_regs(s);
+    wgmma_fence();
 #pragma unroll
-      for (int j = 1; j < 32; ++j) mt = fmaxf(mt, s[j]);
-      // row maximum over both halves
-      float* xs = xch + (t & 1) * 256;
-      xs[g * 128 + rloc] = mt;
-      asm volatile("bar.sync %0, 64;" ::"r"(1 + q) : "memory");
-      mt = fmaxf(mt, xs[(g ^ 1) * 128 + rloc]);
-      const float m_new = fmaxf(m_run, mt * scale);            // scale > 0: max commutes with the scaling; a fully masked half gives -inf
-      const float alpha = __expf(m_run - m_new);               // first tile: exp(-inf) = 0
-      float lsum = 0.f;
+    for (int kk = 0; kk < DK / 8; ++kk) {
+      const uint32_t off = (uint32_t)(kk >> 2) * BLK_BYTES + (uint32_t)(kk & 3) * 32;            // K: [plane][d_k block]
+      const uint32_t qoff = (uint32_t)(kk >> 2) * 2 * BLK_BYTES + (uint32_t)(kk & 3) * 32;       // Q: [plane][d_k block][row block]
+      const uint64_t a_hi = gmma_desc(qa + qoff), a_lo = gmma_desc(qa + 4 * BLK_BYTES + qoff);
+      const uint64_t b_hi = gmma_desc(kt + off), b_lo = gmma_desc(kt + 2 * BLK_BYTES + off);
+      wgmma_tf32_ss_n64(s, a_lo, b_hi, kk != 0 ? 1u : 0u);   // small terms first
+      wgmma_tf32_ss_n64(s, a_hi, b_lo, 1u);
+      wgmma_tf32_ss_n64(s, a_hi, b_hi, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(s);
+    if ((threadIdx.x & 127) == 0) mbar_arrive_local(k_empty + 8 * st);
+    // ---- + rel-pos term, mask, online softmax (rows ra: s[4j], s[4j+1]; rb: s[4j+2], s[4j+3]; key J0 + 8j + 2tq + 0/1)
+    float mt_a = -INFINITY, mt_b = -INFINITY;
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        s[j] = __expf(fmaf(s[j], scale, -m_new));              // masked: exp(-inf) = 0
-        lsum += s[j];
-      }
-      l_run = fmaf(l_run, alpha, lsum);
-      m_run = m_new;
-      if (t > 0) {   // O(t-1) is complete (and P(t-1) has been read): fold it in with the rescale of step t-1
-        ATT_WAIT(o_full + 8 * ((t - 1) & 1), (uint32_t)(((t - 1) >> 1) & 1));
-        tcgen05_fence_after();
-        float ot[32];
-        tmem_ld32_nowait(tmem_base + tlane + TM_O + (uint32_t)((t - 1) & 1) * 64 + cg, ot);
-        tmem_ld_wait();
+    for (int j = 0; j < 8; ++j) {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) o_acc[j] = fmaf(o_acc[j], alpha_prev, ot[j]);
-      }
-      alpha_prev = alpha;
-      {  // P(t) hi / lo -> TMEM
-        float hv[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) hv[j] = espb::tf32_hi(s[j]);
-        tmem_st32(tmem_base + tlane + TM_PHI + cg, hv);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) hv[j] = espb::tf32_lo(s[j], hv[j]);
-        tmem_st32(tmem_base + tlane + TM_PLO + cg, hv);
-        tmem_st_wait();
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_remote(p_full, 0);
+      for (int e = 0; e < 2; ++e) {
+        const int key = J0 + 8 * j + 2 * tq + e;
+        const bool ok = key < len;
+        float va = s[4 * j + e], vb = s[4 * j + 2 + e];
+        if (RELPOS) {
+          if (ok && bd_a) va += __ldg(bd_a + key);
+          if (ok && bd_b) vb += __ldg(bd_b + key);
+        }
+        va = ok ? va : -INFINITY;
+        vb = ok ? vb : -INFINITY;
+        s[4 * j + e] = va; s[4 * j + 2 + e] = vb;
+        mt_a = fmaxf(mt_a, va); mt_b = fmaxf(mt_b, vb);
       }
     }
-    {  // last tile's O, total row sum, normalise, store hi/lo
-      const int t = nkt - 1;
-      float* xs = xch + ((t + 1) & 1) * 256;
-      xs[g * 128 + rloc] = l_run;
-      asm volatile("bar.sync %0, 64;" ::"r"(1 + q) : "memory");
-      const float inv = 1.f / (l_run + xs[(g ^ 1) * 128 + rloc]);
-      ATT_WAIT(o_full + 8 * (t & 1), (uint32_t)((t >> 1) & 1));
-      tcgen05_fence_after();
-      float* o = p.out + ((long long)b * p.T + row) * p.ldo + h * DK + cg;
-      float ot[32];
-      tmem_ld32_nowait(tmem_base + tlane + TM_O + (uint32_t)(t & 1) * 64 + cg, ot);
-      tmem_ld_wait();
-      if (row < p.T) {
+    mt_a = fmaxf(mt_a, __shfl_xor_sync(0xffffffffu, mt_a, 1)); mt_a = fmaxf(mt_a, __shfl_xor_sync(0xffffffffu, mt_a, 2));
+    mt_b = fmaxf(mt_b, __shfl_xor_sync(0xffffffffu, mt_b, 1)); mt_b = fmaxf(mt_b, __shfl_xor_sync(0xffffffffu, mt_b, 2));
+    const float mn_a = fmaxf(m_a, mt_a * scale), mn_b = fmaxf(m_b, mt_b * scale);   // scale > 0: max commutes with the scaling
+    const float al_a = __expf(m_a - mn_a), al_b = __expf(m_b - mn_b);              // first tile: exp(-inf) = 0
+    float ls_a = 0.f, ls_b = 0.f;
 #pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          float4 hi, lo;
-          const float v0 = fmaf(o_acc[j], alpha_prev, ot[j]) * inv, v1 = fmaf(o_acc[j + 1], alpha_prev, ot[j + 1]) * inv;
-          const float v2 = fmaf(o_acc[j + 2], alpha_prev, ot[j + 2]) * inv, v3 = fmaf(o_acc[j + 3], alpha_prev, ot[j + 3]) * inv;
-          hi.x = espb::tf32_hi(v0); hi.y = espb::tf32_hi(v1); hi.z = espb::tf32_hi(v2); hi.w = espb::tf32_hi(v3);
-          lo.x = espb::tf32_lo(v0, hi.x); lo.y = espb::tf32_lo(v1, hi.y); lo.z = espb::tf32_lo(v2, hi.z); lo.w = espb::tf32_lo(v3, hi.w);
-          *reinterpret_cast<float4*>(o + j) = hi;
-          *reinterpret_cast<float4*>(o + p.out_plane + j) = lo;
-        }
+    for (int j = 0; j < 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        s[4 * j + e] = __expf(fmaf(s[4 * j + e], scale, -mn_a));           // masked: exp(-inf) = 0
+        s[4 * j + 2 + e] = __expf(fmaf(s[4 * j + 2 + e], scale, -mn_b));
+        ls_a += s[4 * j + e]; ls_b += s[4 * j + 2 + e];
       }
+    }
+    l_a = fmaf(l_a, al_a, ls_a); l_b = fmaf(l_b, al_b, ls_b);
+    m_a = mn_a; m_b = mn_b;
+    // ---- O(t) = P(t) V(t): P from registers (accumulator layout -> A-fragment layout through quad shuffles)
+    mbar_wait_spin(v_full + 8 * st, ph);
+    const uint32_t vt = v_base + st * KV_STAGE_BYTES;
+    uint32_t ph_hi[8][4], ph_lo[8][4];
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      const float x00 = __shfl_sync(0xffffffffu, s[4 * kk], src0), x01 = __shfl_sync(0xffffffffu, s[4 * kk + 1], src0);
+      const float x10 = __shfl_sync(0xffffffffu, s[4 * kk], src1), x11 = __shfl_sync(0xffffffffu, s[4 * kk + 1], src1);
+      const float y00 = __shfl_sync(0xffffffffu, s[4 * kk + 2], src0), y01 = __shfl_sync(0xffffffffu, s[4 * kk + 3], src0);
+      const float y10 = __shfl_sync(0xffffffffu, s[4 * kk + 2], src1), y11 = __shfl_sync(0xffffffffu, s[4 * kk + 3], src1);
+      const float a[4] = {(tq & 1) ? x01 : x00, (tq & 1) ? y01 : y00, (tq & 1) ? x11 : x10, (tq & 1) ? y11 : y10};
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float hi = espb::tf32_hi(a[i]);
+        ph_hi[kk][i] = __float_as_uint(hi);
+        ph_lo[kk][i] = __float_as_uint(espb::tf32_lo(a[i], hi));
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < 32; ++j) ot[j] = 0.f;
+    fence_regs(ot);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < KB / 8; ++kk) {
+      const uint32_t off = (uint32_t)(kk >> 2) * BLK_BYTES + (uint32_t)(kk & 3) * 32;
+      const uint64_t b_hi = gmma_desc(vt + off), b_lo = gmma_desc(vt + 2 * BLK_BYTES + off);
+      wgmma_tf32_rs_n64(ot, ph_lo[kk], b_hi, kk != 0 ? 1u : 0u);
+      wgmma_tf32_rs_n64(ot, ph_hi[kk], b_lo, 1u);
+      wgmma_tf32_rs_n64(ot, ph_hi[kk], b_hi, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(ot);
+    if ((threadIdx.x & 127) == 0) mbar_arrive_local(v_empty + 8 * st);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      o_acc[4 * j] = fmaf(o_acc[4 * j], al_a, ot[4 * j]); o_acc[4 * j + 1] = fmaf(o_acc[4 * j + 1], al_a, ot[4 * j + 1]);
+      o_acc[4 * j + 2] = fmaf(o_acc[4 * j + 2], al_b, ot[4 * j + 2]); o_acc[4 * j + 3] = fmaf(o_acc[4 * j + 3], al_b, ot[4 * j + 3]);
     }
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  cluster_sync_all();   // the peer may still signal this CTA's barriers / the MMAs may still read this CTA's smem until both are done
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
+  // ---- total row sums over the quad, normalise, store hi / lo
+  l_a += __shfl_xor_sync(0xffffffffu, l_a, 1); l_a += __shfl_xor_sync(0xffffffffu, l_a, 2);
+  l_b += __shfl_xor_sync(0xffffffffu, l_b, 1); l_b += __shfl_xor_sync(0xffffffffu, l_b, 2);
+  const float inv_a = 1.f / l_a, inv_b = 1.f / l_b;
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int row = r ? rb : ra;
+    if (row >= p.T) continue;
+    const float inv = r ? inv_b : inv_a;
+    float* o = p.out + ((long long)b * p.T + row) * p.ldo + h * DK + 2 * tq;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float v0 = o_acc[4 * j + 2 * r] * inv, v1 = o_acc[4 * j + 2 * r + 1] * inv;
+      const float h0 = espb::tf32_hi(v0), h1 = espb::tf32_hi(v1);
+      *reinterpret_cast<float2*>(o + 8 * j) = make_float2(h0, h1);
+      *reinterpret_cast<float2*>(o + p.out_plane + 8 * j) = make_float2(espb::tf32_lo(v0, h0), espb::tf32_lo(v1, h1));
+    }
   }
 }
 
 template <bool RELPOS>
-int launch_flash(const CUtensorMap& tmK, const CUtensorMap& tmV, const CUtensorMap& tmBD, const AttnParams& p, cudaStream_t stream) {
-  constexpr int smem = 2 * KV_STAGES * KV_STAGE_BYTES + (RELPOS ? BD_STAGES * BD_STAGE_BYTES : 0) + 1024 + 256 + 2048;
+int launch_flash(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const AttnParams& p, cudaStream_t stream) {
+  constexpr int smem = Q_BYTES + 2 * KV_STAGES * KV_STAGE_BYTES + 1024 + 256;
   static_assert(smem <= 232448, "dynamic shared memory budget exceeded");
   static bool attr_set = false;
   if (!attr_set) {
@@ -374,7 +275,7 @@ int launch_flash(const CUtensorMap& tmK, const CUtensorMap& tmV, const CUtensorM
     attr_set = true;
   }
   const long long items = (long long)p.B * p.H * p.nqb;
-  flash_attn_kernel<RELPOS><<<dim3((unsigned)(2 * items)), ATT_THREADS, smem, stream>>>(tmK, tmV, tmBD, p);
+  flash_attn_kernel<RELPOS><<<dim3((unsigned)items), ATT_THREADS, smem, stream>>>(tmQ, tmK, tmV, p);
   ESPB_CHECK_LAUNCH();
   return ESPB_OK;
 }
@@ -399,29 +300,28 @@ int espb_flash_attn_f32(const float* q, long long q_off, long long q_plane, long
     espb_set_error("flash_attn: q / out must be 16-byte aligned with strides that are multiples of 4 floats");
     return ESPB_ERR_ARG;
   }
-  CUtensorMap tmK, tmV, tmBD;
+  CUtensorMap tmQ, tmK, tmV;
   int rc;
   {
     long long dims[5] = {DK, T, H, B, 2};
+    long long str[4] = {ldq, DK, (long long)T * ldq, q_plane};
+    if ((rc = espb_make_tensor_map(&tmQ, q, dims, str, 32, 64, 1)) != ESPB_OK) return rc;
+  }
+  {
+    long long dims[5] = {DK, T, H, B, 2};
     long long str[4] = {ldk, DK, (long long)T * ldk, k_plane};
-    if ((rc = espb_make_tensor_map(&tmK, k, dims, str, 32, 32, 1)) != ESPB_OK) return rc;
+    if ((rc = espb_make_tensor_map(&tmK, k, dims, str, 32, 64, 1)) != ESPB_OK) return rc;
   }
   {
     long long dims[5] = {Tp, DK, H, B, 2};
     long long str[4] = {Tp, (long long)DK * Tp, (long long)H * DK * Tp, vt_plane};
-    if ((rc = espb_make_tensor_map(&tmV, vt, dims, str, 32, 32, 1)) != ESPB_OK) return rc;
+    if ((rc = espb_make_tensor_map(&tmV, vt, dims, str, 32, 64, 1)) != ESPB_OK) return rc;
   }
   AttnParams p;
-  p.q = q; p.q_plane = q_plane; p.ldq = ldq; p.lens = lens; p.out = out; p.out_plane = out_plane; p.ldo = ldo;
-  p.B = B; p.H = H; p.T = T; p.nqb = (T + 255) / 256; p.scale = 1.0f / sqrtf((float)dk);
-  if (bd) {
-    long long dims[5] = {Rp, T, H, B, 1};
-    long long str[4] = {Rp, (long long)T * Rp, (long long)H * T * Rp, 0};
-    if ((rc = espb_make_tensor_map(&tmBD, bd, dims, str, BD_COLS, 32, 0)) != ESPB_OK) return rc;
-    return launch_flash<true>(tmK, tmV, tmBD, p, stream);
-  }
-  tmBD = tmK;
-  return launch_flash<false>(tmK, tmV, tmBD, p, stream);
+  p.q = q; p.q_plane = q_plane; p.ldq = ldq; p.lens = lens; p.bd = bd; p.Rp = Rp; p.out = out; p.out_plane = out_plane; p.ldo = ldo;
+  p.B = B; p.H = H; p.T = T; p.nqb = (T + QB - 1) / QB; p.scale = 1.0f / sqrtf((float)dk);
+  if (bd) return launch_flash<true>(tmQ, tmK, tmV, p, stream);
+  return launch_flash<false>(tmQ, tmK, tmV, p, stream);
 }
 
 }  // extern "C"

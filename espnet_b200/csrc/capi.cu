@@ -41,7 +41,7 @@ int espb_device_sm(int* major, int* minor) {
   return ESPB_OK;
 }
 
-// use_tc = 1: tcgen05 3xTF32 kernel (TMA needs 16-byte aligned strides/bases); 0: SIMT fp32 kernel.
+// use_tc = 1: wgmma 3xTF32 kernel, 2: the same with chunked fp32 promotion (TMA needs 16-byte aligned strides/bases); 0: SIMT fp32 kernel.
 int espb_gemm_f32(const EspbGemmDesc* d, int use_tc, cudaStream_t stream) {
   if (!d) { espb_set_error("gemm: null descriptor"); return ESPB_ERR_ARG; }
   return use_tc ? espb_gemm_tc_launch(*d, stream, use_tc == 2 ? 2 : 1) : espb_gemm_simt_launch(*d, stream);

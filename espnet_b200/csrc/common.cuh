@@ -1,4 +1,4 @@
-// Shared device helpers for the espnet_b200 CUDA library (sm_100a only).
+// Shared device helpers for the espnet_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -22,7 +22,7 @@ constexpr int ACT_NONE = 0, ACT_RELU = 1, ACT_SWISH = 2;
 
 // Programmatic dependent launch for the launch-latency-bound decode step (one beam-search step is ~80 small dependent kernels).
 // A kernel launched through launch_pdl may become resident while its stream predecessor still runs; it must execute pdl_wait()
-// before its first global-memory access (setup that touches only shared memory / TMEM / barriers may precede it).  pdl_trigger()
+// before its first global-memory access (setup that touches only shared memory / barriers may precede it).  pdl_trigger()
 // lets the next kernel in the stream do the same.  Every kernel of the chain waits before it completes, so completion order --
 // and with it every read-after-write / write-after-read dependency of plain stream order -- is preserved transitively.
 // ESPB_PDL=0 launches with full stream serialisation; griddepcontrol.* are no-ops then.
@@ -43,7 +43,7 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 
 // 3xTF32 operand split: hi keeps the top 19 bits (sign, 8 exp, 10 mantissa) of the fp32 value,
 // lo = x - hi is exactly representable in fp32; both planes are stored as fp32 words whose low
-// 13 bits are zero, so tcgen05 kind::tf32 consumes them without rounding ambiguity.
+// 13 bits are zero, so the tf32 wgmma consumes them without rounding ambiguity.
 __device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
 __device__ __forceinline__ float tf32_lo(float x, float hi) { return __uint_as_float(__float_as_uint(x - hi) & 0xFFFFE000u); }
 

@@ -599,7 +599,7 @@ int espb_relpos_softmax_f32(const float* ac, const float* bd, int B, int H, int 
                             long long probs_plane, cudaStream_t stream) {
   long long rows = (long long)B * H * T;
   const unsigned grid = (unsigned)((rows + 7) / 8);
-  // (a register-resident single-pass variant <NV> measured slower on B200: 3.5 ms vs 2.6 ms at T=937 -- lower occupancy; kept for short rows)
+  // (a register-resident single-pass variant <NV> has lower occupancy; kept for short rows)
   if (T <= 128) relpos_softmax_kernel<4><<<grid, 256, 0, stream>>>(ac, bd, B, H, T, Tp, Rp, lens, sqrt_dk, probs, probs_plane);
   else if ((Tp & 3) == 0 && (probs_plane & 3) == 0 && (reinterpret_cast<uintptr_t>(ac) & 15) == 0 && (reinterpret_cast<uintptr_t>(probs) & 15) == 0 &&
            (size_t)8 * Tp * sizeof(float) <= 48 * 1024 && !getenv("ESPB_SOFTMAX_3PASS"))

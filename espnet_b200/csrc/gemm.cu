@@ -1,11 +1,11 @@
-// Error-compensated 3xTF32 GEMM on the 5th-gen tensor cores (tcgen05.mma kind::tf32, fp32
-// accumulators in TMEM, operands staged by TMA with 128B swizzle), plus a SIMT fp32 GEMM with the
-// same descriptor (validator for the tensor-core path and path for shapes TMA cannot address).
+// Error-compensated 3xTF32 GEMM on the Hopper tensor cores (wgmma tf32, fp32 accumulators in registers, operands staged by TMA
+// with 128B swizzle), plus a SIMT fp32 GEMM with the same descriptor (validator for the tensor-core path and path for shapes TMA
+// cannot address).
 //
-// Warp roles per CTA (192 threads, one 128 x BN output tile):
-//   warp 0   : TMA producer (one elected lane)      -> full[s]
-//   warp 1   : TMEM allocator + MMA issuer (one lane) -> empty[s] / tmem_full via tcgen05.commit
-//   warps 2-5: epilogue, TMEM -> registers -> global (bias / activation / residual / hi-lo split)
+// Warp roles per CTA (288 threads, one 128 x BN output tile):
+//   warps 0-7: two consumer warpgroups; warpgroup g issues the wgmma for rows [64g, 64g+64) of the tile and runs their epilogue
+//              (bias / activation / residual / hi-lo split) straight from the accumulator registers
+//   warp 8   : TMA producer (one elected lane) -> full[s]; the consumers release a stage through empty[s] once its MMAs retired
 #include <cuda.h>
 #include <limits.h>
 #include <stdio.h>
@@ -22,7 +22,10 @@ using namespace espb::tc;
 constexpr int BM = 128;
 constexpr int BK = 32;                  // 32 fp32 = 128 B = one swizzle row
 constexpr int A_TILE_BYTES = BM * 128;  // one plane
-constexpr int NUM_THREADS = 192;
+constexpr int NUM_THREADS = 288;
+// Chunked promotion (version 2): K is walked in chunks of CHUNK_KB k-blocks that accumulate in a fresh wgmma accumulator, which is
+// then added into an fp32 register accumulator with round-to-nearest, so the long accumulation chain does not run in the tensor core.
+constexpr int CHUNK_KB = 4;
 
 // ------------------------------------------------------------------ shared epilogue
 struct EpiArgs {
@@ -40,100 +43,72 @@ __device__ __forceinline__ float epi_value(const EpiArgs& e, float acc, long lon
 }
 
 // ------------------------------------------------------------------ tensor-core kernel
-// Epilogue of one 32-column chunk of a 128-row 1-CTA tile (the thread owns row `row`, v[] holds its 32 accumulators): bias, activation,
-// alpha / residual, optional hi / lo split; 128-bit accesses when the layout allows.  Shared by the 1-CTA, multicast and split-K kernels.
-__device__ __forceinline__ void epi_store_chunk32(const EpiArgs& e, float (&v)[32], int row, bool row_ok, int col0, int N, bool vec_ok, bool r_vec_ok) {
+// rel-pos band (EspbGemmDesc::band_t): a tile of rows [m0, m0+bm) x columns [n0, n0+bn) is needed iff it intersects
+// { (m, n) : T-1-m <= n <= 2T-2-m }.
+__device__ __forceinline__ bool band_skip(int T, int m0, int bm, int n0, int bn) {
+  if (T <= 0) return false;
+  return (n0 + bn - 1 < T - 1 - (m0 + bm - 1)) || (n0 > 2 * T - 2 - m0);
+}
+
+template <int BN>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc, uint32_t accum) {
+  if constexpr (BN == 128) wgmma_tf32_ss_n128(d, adesc, bdesc, accum);
+  else wgmma_tf32_ss_n64(d, adesc, bdesc, accum);
+}
+
+// Epilogue of two horizontally adjacent accumulator elements (row, col) and (row, col + 1).
+__device__ __forceinline__ void epi_store2(const EpiArgs& e, int row, int col, float v0, float v1, int M, int N, bool vec_ok) {
+  if (row >= M || col >= N) return;
   float* crow = e.C + (long long)row * e.ldc;
-  if (!row_ok || col0 >= N) return;   // nothing to store for this lane / column chunk (tile overhang)
-  if (vec_ok && col0 + 32 <= N) {
-    // residual (may alias the output: x += ...) and bias are fetched up front with 128-bit loads, so the 8 loads are in flight
-    // together instead of one dependent load -> store round trip per element
-    float rres[32];
-    if (e.R && r_vec_ok) {
-      const float4* rp4 = reinterpret_cast<const float4*>(e.R + (long long)row * e.ldr + col0);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { const float4 t = rp4[j]; rres[4 * j] = t.x; rres[4 * j + 1] = t.y; rres[4 * j + 2] = t.z; rres[4 * j + 3] = t.w; }
+  const bool two = col + 1 < N;
+  const float t0 = epi_value(e, v0, row, col), t1 = two ? epi_value(e, v1, row, col + 1) : 0.f;
+  if (vec_ok && two) {
+    if (e.split_out) {
+      const float h0 = espb::tf32_hi(t0), h1 = espb::tf32_hi(t1);
+      *reinterpret_cast<float2*>(crow + col) = make_float2(h0, h1);
+      *reinterpret_cast<float2*>(crow + e.c_plane + col) = make_float2(espb::tf32_lo(t0, h0), espb::tf32_lo(t1, h1));
     } else {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) rres[j] = e.R ? e.R[(long long)row * e.ldr + col0 + j] : 0.f;
+      *reinterpret_cast<float2*>(crow + col) = make_float2(t0, t1);
     }
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      float x = v[j];
-      if (e.bias) x += __ldg(e.bias + col0 + j);
-      x = espb::apply_act_acc(x, e.act);
-      v[j] = fmaf(e.alpha, x, rres[j]);
-    }
-#pragma unroll
-    for (int j = 0; j < 32; j += 4) {
-      float4 o, l;
-      const float t0 = v[j], t1 = v[j + 1], t2 = v[j + 2], t3 = v[j + 3];
-      if (e.split_out) {
-        o.x = espb::tf32_hi(t0); o.y = espb::tf32_hi(t1); o.z = espb::tf32_hi(t2); o.w = espb::tf32_hi(t3);
-        l.x = espb::tf32_lo(t0, o.x); l.y = espb::tf32_lo(t1, o.y); l.z = espb::tf32_lo(t2, o.z); l.w = espb::tf32_lo(t3, o.w);
-        *reinterpret_cast<float4*>(crow + col0 + j) = o;
-        *reinterpret_cast<float4*>(crow + e.c_plane + col0 + j) = l;
-      } else {
-        o.x = t0; o.y = t1; o.z = t2; o.w = t3;
-        *reinterpret_cast<float4*>(crow + col0 + j) = o;
-      }
-    }
-  } else {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      const int col = col0 + j;
-      if (col < N) {
-        const float t = epi_value(e, v[j], row, col);
-        if (e.split_out) {
-          const float h = espb::tf32_hi(t);
-          crow[col] = h; crow[e.c_plane + col] = espb::tf32_lo(t, h);
-        } else {
-          crow[col] = t;
-        }
-      }
-    }
+    return;
+  }
+  const float t[2] = {t0, t1};
+  for (int i = 0; i < (two ? 2 : 1); ++i) {
+    if (e.split_out) { const float h = espb::tf32_hi(t[i]); crow[col + i] = h; crow[e.c_plane + col + i] = espb::tf32_lo(t[i], h); }
+    else crow[col + i] = t[i];
   }
 }
 
-template <int BN, int STAGES>
+template <int BN, int STAGES, bool PROMOTE>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, EspbGemmDesc p, int bxm, int bym, int axm, int aym) {
   constexpr int B_TILE_BYTES = BN * 128;
   constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
+  constexpr int NR = BN / 2;   // accumulator registers per thread: a 64 x BN warpgroup tile over 128 threads
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + STAGES * STAGE_BYTES;  // full[STAGES], empty[STAGES], tmem_full, tmem_ptr
-  const uint32_t full_bar = bar_base, empty_bar = bar_base + 8 * STAGES, tmem_full_bar = bar_base + 16 * STAGES;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(smem_raw + (bar_base - smem_u32(smem_raw)) + 16 * STAGES + 8);
+  const uint32_t full_bar = smem_base + STAGES * STAGE_BYTES, empty_bar = full_bar + 8 * STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
   const int bx = blockIdx.z % p.nbx, by = blockIdx.z / p.nbx;
   const int num_kb = (p.K + BK - 1) / BK;
-  if (p.band_t > 0 && ((n0 + BN - 1 < p.band_t - 1 - (m0 + BM - 1)) || (n0 > 2 * p.band_t - 2 - m0))) {   // tile outside the rel-pos band
+  if (band_skip(p.band_t, m0, BM, n0, BN)) {   // tile outside the rel-pos band
     espb::pdl_wait();
     return;
   }
 
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 1); }
-    mbar_init(tmem_full_bar, 1);
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 2); }   // empty: one arrival per consumer warpgroup
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"((uint32_t)BN) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  espb::pdl_trigger();   // barriers, TMEM and descriptors are ready: the next kernel may start its own setup
+  espb::pdl_trigger();   // barriers and descriptors are ready: the next kernel may start its own setup
   espb::pdl_wait();      // first global access (TMA loads of A / B) follows
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (elect_one_sync()) {   // one lane, known to ptxas: uniform-datapath issue without per-instruction waterfall loops
       const int cblk = (p.a_mode == 1) ? p.cv_cin / BK : 0;
       for (int kb = 0; kb < num_kb; ++kb) {
@@ -159,652 +134,53 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         tma_load_5d(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, &tmB, fb, kb * BK, n0, bx * bxm, by * bym, 1);
       }
     }
-  } else if (warp == 1) {
-    if (elect_one_sync()) {   // one lane, known to ptxas: uniform-datapath issue without per-instruction waterfall loops
-      // instruction descriptor: D=f32 (bit 4), A=B=tf32 (2 at bits 7,10), both K-major, N>>3 at bit 17, M>>4 at bit 24
-      const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        mbar_wait(full_bar + 8 * s, ph);
-        tcgen05_fence_after();
-        const uint32_t sa = smem_base + s * STAGE_BYTES;
+    return;
+  }
+
+  const int wg = warp >> 2;
+  float acc[NR], part[NR];
 #pragma unroll
-        for (int k = 0; k < BK / 8; ++k) {  // UMMA_K = 8 tf32 = 32 bytes
-          const uint64_t a_hi = umma_desc(sa + k * 32), a_lo = umma_desc(sa + A_TILE_BYTES + k * 32);
-          const uint64_t b_hi = umma_desc(sa + 2 * A_TILE_BYTES + k * 32);
-          const uint64_t b_lo = umma_desc(sa + 2 * A_TILE_BYTES + B_TILE_BYTES + k * 32);
-          mma_tf32(tmem_base, a_lo, b_hi, idesc, (kb | k) != 0);  // small terms first
-          mma_tf32(tmem_base, a_hi, b_lo, idesc, 1);
-          mma_tf32(tmem_base, a_hi, b_hi, idesc, 1);
-        }
-        tcgen05_commit(empty_bar + 8 * s);  // frees the smem stage once these MMAs retire
-      }
-      tcgen05_commit(tmem_full_bar);
+  for (int i = 0; i < NR; ++i) { acc[i] = 0.f; part[i] = 0.f; }
+  for (int kb = 0; kb < num_kb; ++kb) {
+    const int s = kb % STAGES;
+    mbar_wait(full_bar + 8 * s, (kb / STAGES) & 1);
+    const uint32_t sa = smem_base + s * STAGE_BYTES + wg * 64 * 128;   // this warpgroup's 64 rows of A (8 KB: swizzle atoms stay aligned)
+    const uint32_t sb = smem_base + s * STAGE_BYTES + 2 * A_TILE_BYTES;
+    const bool fresh = PROMOTE ? (kb % CHUNK_KB == 0) : (kb == 0);
+    fence_regs(part);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 8; ++k) {   // 8 tf32 = 32 bytes per MMA
+      const uint64_t a_hi = gmma_desc(sa + k * 32), a_lo = gmma_desc(sa + A_TILE_BYTES + k * 32);
+      const uint64_t b_hi = gmma_desc(sb + k * 32), b_lo = gmma_desc(sb + B_TILE_BYTES + k * 32);
+      wgmma_tf32<BN>(part, a_lo, b_hi, (fresh && k == 0) ? 0u : 1u);   // small terms first
+      wgmma_tf32<BN>(part, a_hi, b_lo, 1u);
+      wgmma_tf32<BN>(part, a_hi, b_hi, 1u);
     }
-  } else {
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    mbar_wait(tmem_full_bar, 0);
-    tcgen05_fence_after();
-    const int row = m0 + q * 32 + lane;
-    const bool row_ok = row < p.M;
-    EpiArgs e;
-    const long long coff = (long long)by * p.sc_y + (long long)bx * p.sc_x;
-    e.C = p.C + coff; e.c_plane = p.c_plane; e.ldc = p.ldc; e.split_out = p.split_out;
-    e.bias = p.bias ? p.bias + (long long)bx * p.sbias_x : nullptr; e.R = p.R ? p.R + (long long)by * p.sr_y + (long long)bx * p.sr_x : nullptr;
-    e.ldr = p.ldr; e.alpha = p.alpha; e.act = p.act;
-    const bool vec_ok = ((p.ldc & 3) == 0) && ((coff & 3) == 0) && ((p.c_plane & 3) == 0) &&
-                        ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
-    const bool r_vec_ok = p.R && ((p.ldr & 3) == 0) && ((((long long)by * p.sr_y + (long long)bx * p.sr_x) & 3) == 0) &&
-                          ((reinterpret_cast<uintptr_t>(p.R) & 15) == 0);
-#pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-      float v[32];
-      __syncwarp();
-      tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), v);
-      epi_store_chunk32(e, v, row, row_ok, n0 + c * 32, p.N, vec_ok, r_vec_ok);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(part);
+    if ((threadIdx.x & 127) == 0) mbar_arrive_local(empty_bar + 8 * s);   // this warpgroup no longer reads the stage
+    if (PROMOTE && (kb % CHUNK_KB == CHUNK_KB - 1 || kb == num_kb - 1)) {
+#pragma unroll
+      for (int i = 0; i < NR; ++i) acc[i] += part[i];
     }
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)BN) : "memory");
-  }
-}
 
-// ------------------------------------------------------------------ 1-CTA tiles with the A operand multicast across a cluster
-// Small-M (decode-step) problems are bound by the per-SM TMA ingest rate (~32 B/cycle): the MC CTAs of a cluster compute MC
-// neighbouring n-tiles of the same m-tile, each fetches 1/MC of the A tile and multicasts it to all of them, so every CTA ingests
-// A/MC + B instead of A + B.  A stage is refilled only after all MC consumers released it (their tcgen05.commit arrives on the
-// empty barrier of every CTA of the cluster).
-template <int BN, int STAGES, int MC>
-__global__ void __cluster_dims__(1, MC, 1) __launch_bounds__(NUM_THREADS, 1)
-gemm_tf32x3_mc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, EspbGemmDesc p, int bxm, int bym, int axm, int aym) {
-  constexpr int B_TILE_BYTES = BN * 128;
-  constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + STAGES * STAGE_BYTES;  // full[STAGES], empty[STAGES], tmem_full, tmem_ptr
-  const uint32_t full_bar = bar_base, empty_bar = bar_base + 8 * STAGES, tmem_full_bar = bar_base + 16 * STAGES;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(smem_raw + (bar_base - smem_u32(smem_raw)) + 16 * STAGES + 8);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
-  const int bx = blockIdx.z % p.nbx, by = blockIdx.z / p.nbx;
-  const int num_kb = (p.K + BK - 1) / BK;
-  const uint32_t rank = cluster_ctarank_v();            // position of this n-tile inside its cluster
-  constexpr uint16_t MASK = (uint16_t)((1u << MC) - 1);
-  constexpr int SLICE_ROWS = BM / MC, SLICE_BYTES = SLICE_ROWS * 128;
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, MC); }
-    mbar_init(tmem_full_bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"((uint32_t)BN) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  cluster_sync_all_v();     // every CTA's barriers are initialised before any multicast / remote arrive can reach them
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  espb::pdl_trigger();
-  espb::pdl_wait();
-
-  if (warp == 0) {
-    if (elect_one_sync()) {   // one lane, known to ptxas: uniform-datapath issue without per-instruction waterfall loops
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        mbar_wait(empty_bar + 8 * s, ph ^ 1);
-        const uint32_t fb = full_bar + 8 * s;
-        mbar_expect_tx(fb, STAGE_BYTES);
-        const uint32_t sa = smem_base + s * STAGE_BYTES;
-        {
-          const int ko = (p.kob > 0) ? kb / p.kob : 0;
-          const int ki = (p.kob > 0) ? kb % p.kob : kb;
-          const int mrow = m0 + (int)rank * SLICE_ROWS;          // this CTA's slice of the shared A tile, delivered to all MC CTAs
-          tma_load_5d_mc(sa + rank * SLICE_BYTES, &tmA, fb, ki * BK, mrow, bx * axm + ko, by * aym, 0, MASK);
-          tma_load_5d_mc(sa + A_TILE_BYTES + rank * SLICE_BYTES, &tmA, fb, ki * BK, mrow, bx * axm + ko, by * aym, 1, MASK);
-        }
-        tma_load_5d(sa + 2 * A_TILE_BYTES, &tmB, fb, kb * BK, n0, bx * bxm, by * bym, 0);
-        tma_load_5d(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, &tmB, fb, kb * BK, n0, bx * bxm, by * bym, 1);
-      }
-    }
-  } else if (warp == 1) {
-    if (elect_one_sync()) {   // one lane, known to ptxas: uniform-datapath issue without per-instruction waterfall loops
-      // instruction descriptor: D=f32 (bit 4), A=B=tf32 (2 at bits 7,10), both K-major, N>>3 at bit 17, M>>4 at bit 24
-      const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        mbar_wait(full_bar + 8 * s, ph);
-        tcgen05_fence_after();
-        const uint32_t sa = smem_base + s * STAGE_BYTES;
+  EpiArgs e;
+  const long long coff = (long long)by * p.sc_y + (long long)bx * p.sc_x;
+  const long long roff = (long long)by * p.sr_y + (long long)bx * p.sr_x;
+  e.C = p.C + coff; e.c_plane = p.c_plane; e.ldc = p.ldc; e.split_out = p.split_out;
+  e.bias = p.bias ? p.bias + (long long)bx * p.sbias_x : nullptr; e.R = p.R ? p.R + roff : nullptr;
+  e.ldr = p.ldr; e.alpha = p.alpha; e.act = p.act;
+  const bool vec_ok = ((p.ldc & 1) == 0) && ((coff & 1) == 0) && ((p.c_plane & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 7) == 0);
+  const int row = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int col = n0 + 2 * (lane & 3);
 #pragma unroll
-        for (int k = 0; k < BK / 8; ++k) {  // UMMA_K = 8 tf32 = 32 bytes
-          const uint64_t a_hi = umma_desc(sa + k * 32), a_lo = umma_desc(sa + A_TILE_BYTES + k * 32);
-          const uint64_t b_hi = umma_desc(sa + 2 * A_TILE_BYTES + k * 32);
-          const uint64_t b_lo = umma_desc(sa + 2 * A_TILE_BYTES + B_TILE_BYTES + k * 32);
-          mma_tf32(tmem_base, a_lo, b_hi, idesc, (kb | k) != 0);  // small terms first
-          mma_tf32(tmem_base, a_hi, b_lo, idesc, 1);
-          mma_tf32(tmem_base, a_hi, b_hi, idesc, 1);
-        }
-        tcgen05_commit_mc(empty_bar + 8 * s, MASK);  // releases this stage in every CTA of the cluster once these MMAs retire
-      }
-      tcgen05_commit(tmem_full_bar);
-    }
-  } else {
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    mbar_wait(tmem_full_bar, 0);
-    tcgen05_fence_after();
-    const int row = m0 + q * 32 + lane;
-    const bool row_ok = row < p.M;
-    EpiArgs e;
-    const long long coff = (long long)by * p.sc_y + (long long)bx * p.sc_x;
-    e.C = p.C + coff; e.c_plane = p.c_plane; e.ldc = p.ldc; e.split_out = p.split_out;
-    e.bias = p.bias ? p.bias + (long long)bx * p.sbias_x : nullptr; e.R = p.R ? p.R + (long long)by * p.sr_y + (long long)bx * p.sr_x : nullptr;
-    e.ldr = p.ldr; e.alpha = p.alpha; e.act = p.act;
-    const bool vec_ok = ((p.ldc & 3) == 0) && ((coff & 3) == 0) && ((p.c_plane & 3) == 0) &&
-                        ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
-    const bool r_vec_ok = p.R && ((p.ldr & 3) == 0) && ((((long long)by * p.sr_y + (long long)bx * p.sr_x) & 3) == 0) &&
-                          ((reinterpret_cast<uintptr_t>(p.R) & 15) == 0);
-#pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-      float v[32];
-      __syncwarp();
-      tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), v);
-      epi_store_chunk32(e, v, row, row_ok, n0 + c * 32, p.N, vec_ok, r_vec_ok);
-    }
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  cluster_sync_all_v();     // peers may still multicast into / arrive on this CTA's smem until all are done
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)BN) : "memory");
-  }
-}
-
-// ------------------------------------------------------------------ 1-CTA tiles with K split across a cluster (decode-step GEMMs)
-// A decode step multiplies a few hundred rows by a weight matrix: there are far fewer 128 x BN tiles than SMs and each CTA's time is
-// the serial walk over K (TMA ingest + barrier round trips per k-block).  The SK CTAs of a cluster (cluster dim z) each accumulate
-// 1/SK of the k-blocks of the SAME output tile in their own TMEM; the partial tiles are then reduce-scattered through distributed
-// shared memory: CTA r finalises the 32-column chunks c with c % SK == r, adding the other CTAs' partials in ascending rank order
-// (fixed order -> deterministic) before the usual bias / activation / residual / hi-lo split epilogue.
-template <int BN, int STAGES, int SK>
-__global__ void __cluster_dims__(1, 1, SK) __launch_bounds__(NUM_THREADS, 1)
-gemm_tf32x3_sk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, EspbGemmDesc p) {
-  constexpr int B_TILE_BYTES = BN * 128;
-  constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
-  constexpr int NCHUNK = BN / 32;
-  static_assert(STAGES * STAGE_BYTES >= BN * BM * 4, "partial-tile staging must fit in the pipeline buffers");
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + STAGES * STAGE_BYTES;  // full[STAGES], empty[STAGES], tmem_full, tmem_ptr
-  const uint32_t full_bar = bar_base, empty_bar = bar_base + 8 * STAGES, tmem_full_bar = bar_base + 16 * STAGES;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(smem_raw + (bar_base - smem_u32(smem_raw)) + 16 * STAGES + 8);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
-  const uint32_t rank = cluster_ctarank_v();            // == blockIdx.z: which K slice
-  const int num_kb_all = (p.K + BK - 1) / BK;
-  const int kb_per = (num_kb_all + SK - 1) / SK;
-  const int kb0 = (int)rank * kb_per;
-  const int nkb = min(num_kb_all, kb0 + kb_per) - kb0;   // >= 1 (checked on the host)
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 1); }
-    mbar_init(tmem_full_bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"((uint32_t)BN) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  espb::pdl_trigger();
-  espb::pdl_wait();
-  const int q = warp & 3;                                // TMEM lane quarter of an epilogue warp
-  // staging layout: [chunk][j/4][row 0..127][4 floats] -> 128-bit conflict-free writes (lane = row) and 128-bit remote reads
-  const uint32_t stg_lane = smem_base + (uint32_t)(q * 32 + lane) * 16u;
-
-  if (warp == 0) {
-    if (elect_one_sync()) {   // one lane, known to ptxas: uniform-datapath issue without per-instruction waterfall loops
-      for (int i = 0; i < nkb; ++i) {
-        const int s = i % STAGES;
-        const uint32_t ph = (i / STAGES) & 1;
-        mbar_wait(empty_bar + 8 * s, ph ^ 1);
-        const uint32_t fb = full_bar + 8 * s;
-        mbar_expect_tx(fb, STAGE_BYTES);
-        const uint32_t sa = smem_base + s * STAGE_BYTES;
-        const int k0 = (kb0 + i) * BK;
-        tma_load_5d(sa, &tmA, fb, k0, m0, 0, 0, 0);
-        tma_load_5d(sa + A_TILE_BYTES, &tmA, fb, k0, m0, 0, 0, 1);
-        tma_load_5d(sa + 2 * A_TILE_BYTES, &tmB, fb, k0, n0, 0, 0, 0);
-        tma_load_5d(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, &tmB, fb, k0, n0, 0, 0, 1);
-      }
-    }
-  } else if (warp == 1) {
-    if (elect_one_sync()) {   // one lane, known to ptxas: uniform-datapath issue without per-instruction waterfall loops
-      const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-      for (int i = 0; i < nkb; ++i) {
-        const int s = i % STAGES;
-        const uint32_t ph = (i / STAGES) & 1;
-        mbar_wait(full_bar + 8 * s, ph);
-        tcgen05_fence_after();
-        const uint32_t sa = smem_base + s * STAGE_BYTES;
-#pragma unroll
-        for (int k = 0; k < BK / 8; ++k) {  // UMMA_K = 8 tf32 = 32 bytes
-          const uint64_t a_hi = umma_desc(sa + k * 32), a_lo = umma_desc(sa + A_TILE_BYTES + k * 32);
-          const uint64_t b_hi = umma_desc(sa + 2 * A_TILE_BYTES + k * 32);
-          const uint64_t b_lo = umma_desc(sa + 2 * A_TILE_BYTES + B_TILE_BYTES + k * 32);
-          mma_tf32(tmem_base, a_lo, b_hi, idesc, (i | k) != 0);  // small terms first
-          mma_tf32(tmem_base, a_hi, b_lo, idesc, 1);
-          mma_tf32(tmem_base, a_hi, b_hi, idesc, 1);
-        }
-        tcgen05_commit(empty_bar + 8 * s);
-      }
-      tcgen05_commit(tmem_full_bar);   // all MMAs retired: accumulators complete, pipeline smem no longer read
-    }
-  } else {
-    // phase 1: park the chunks other CTAs finalise in this CTA's (now idle) pipeline buffers
-    mbar_wait(tmem_full_bar, 0);
-    tcgen05_fence_after();
-#pragma unroll 1
-    for (int c = 0; c < NCHUNK; ++c) {
-      if ((uint32_t)(c % SK) == rank) continue;          // warp-uniform
-      float v[32];
-      __syncwarp();
-      tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), v);
-#pragma unroll
-      for (int j4 = 0; j4 < 8; ++j4) {
-        const uint32_t a = stg_lane + (uint32_t)((c * 8 + j4) * BM) * 16u;
-        asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(a), "f"(v[4 * j4]), "f"(v[4 * j4 + 1]), "f"(v[4 * j4 + 2]), "f"(v[4 * j4 + 3])
-                     : "memory");
-      }
-    }
-  }
-  __syncwarp();
-  cluster_sync_all_v();     // release/acquire: every CTA's parked partials are visible cluster-wide
-
-  if (warp >= 2) {
-    const int row = m0 + q * 32 + lane;
-    const bool row_ok = row < p.M;
-    EpiArgs e;
-    e.C = p.C; e.c_plane = p.c_plane; e.ldc = p.ldc; e.split_out = p.split_out;
-    e.bias = p.bias; e.R = p.R; e.ldr = p.ldr; e.alpha = p.alpha; e.act = p.act;
-    const bool vec_ok = ((p.ldc & 3) == 0) && ((p.c_plane & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
-    const bool r_vec_ok = p.R && ((p.ldr & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.R) & 15) == 0);
-#pragma unroll 1
-    for (int c = 0; c < NCHUNK; ++c) {
-      if ((uint32_t)(c % SK) != rank) continue;
-      float v[32];
-      __syncwarp();
-      tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), v);
-#pragma unroll
-      for (int r = 0; r < SK; ++r) {
-        if ((uint32_t)r == rank) continue;
-#pragma unroll
-        for (int j4 = 0; j4 < 8; ++j4) {
-          const float4 t = ld_dsmem_f4(stg_lane + (uint32_t)((c * 8 + j4) * BM) * 16u, (uint32_t)r);
-          v[4 * j4] += t.x; v[4 * j4 + 1] += t.y; v[4 * j4 + 2] += t.z; v[4 * j4 + 3] += t.w;
-        }
-      }
-      epi_store_chunk32(e, v, row, row_ok, n0 + c * 32, p.N, vec_ok, r_vec_ok);
-    }
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  cluster_sync_all_v();     // peers may still read this CTA's parked partials until all are done
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)BN) : "memory");
-  }
-}
-
-// ------------------------------------------------------------------ tensor-core kernel v2: CTA pair + chunked promotion
-// cta_group::2: a cluster of two CTAs computes a 256 x BN tile (UMMA M=256); each CTA stages its own 128 rows of A and
-// its half (BN/2 rows) of B, so per-SM L2->smem traffic per MMA is halved against the 1-CTA kernel. The fp32 accumulator of
-// the tensor core truncates on every accumulation step, so K is walked in chunks of CHUNK_KB k-blocks that accumulate in
-// one of two TMEM buffers (restart with accumulate=0) while 8 epilogue warps add the previous chunk into fp32 registers
-// with round-to-nearest: the long accumulation chain runs on CUDA cores, the products on tensor cores.
-//   warp 0: TMA producer (each CTA loads its halves; both signal the leader CTA's full barrier)
-//   warp 1: TMEM alloc (both CTAs) + MMA issue (leader CTA only)
-//   warps 2-9: epilogue; warp e owns TMEM lanes 32*(e%4).. and columns (e/4)*BN/2 ..
-// CTA-pair kernel: warp 0 TMA, warp 1 MMA, EW epilogue warps (64 + 32 * EW threads)
-constexpr int CHUNK_KB = 4;
-
-// rel-pos band (EspbGemmDesc::band_t): a tile of rows [m0, m0+bm) x columns [n0, n0+bn) is needed iff it intersects
-// { (m, n) : T-1-m <= n <= 2T-2-m }.
-__constant__ int c_band_blocks = 1;   // 0 (ESPB_GEMM_BAND_TILES_ONLY=1): skip whole tiles only, store every 32 x 32 block of a computed tile (A/B measurements)
-__device__ __forceinline__ bool band_skip(int T, int m0, int bm, int n0, int bn) {
-  if (T <= 0) return false;
-  return (n0 + bn - 1 < T - 1 - (m0 + bm - 1)) || (n0 > 2 * T - 2 - m0);
-}
-
-// Dynamic read of a register array (cold scalar path only): unrolled compare/select keeps `acc` in registers.
-template <int N>
-__device__ __forceinline__ float acc_at(const float (&acc)[N], int idx) {
-  float r = 0.f;
-#pragma unroll
-  for (int i = 0; i < N; ++i) r = (i == idx) ? acc[i] : r;
-  return r;
-}
-
-// ACT / SPLIT are compile-time so that the 128-bit epilogue path carries no per-element branches.
-template <int BN, int STAGES, int ACT, bool SPLIT, bool PLAIN, int EW>   // EW: epilogue warps (8 or 16: 16 halves the accumulator registers per thread); PLAIN: no bias / residual / scaling (the attention score and context products)
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(64 + 32 * EW, 1)
-gemm_tf32x3_2cta_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, EspbGemmDesc p, int bxm, int bym, int axm, int aym) {
-  constexpr int BH = BN / 2;                      // B rows staged by each CTA
-  constexpr int B_TILE_BYTES = BH * 128;
-  constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
-  constexpr int CW = BN * 4 / EW;                 // accumulator columns per epilogue warp (EW / 4 column groups x 4 TMEM lane quarters)
-  constexpr int XR = 128 / EW;                    // rows of the per-warp transpose buffer: a 32-row block goes through it in 32 / XR passes
-  constexpr int NH = 32 / XR, ITS = XR / 4;
-  constexpr int LDW = (EW == 16) ? 16 : 32;       // columns per tcgen05.ld of the promotion loop (16 warps run at 112 registers)
-  constexpr int XP_FLOATS = XR * 36;              // per-warp transpose buffer of the coalescing epilogue (XR rows x 32 cols, padded)
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t xp_base = smem_base + STAGES * STAGE_BYTES;            // 8 warps x [32][33] floats
-  const uint32_t bar_base = xp_base + EW * XP_FLOATS * 4;
-  const uint32_t full_bar = bar_base, empty_bar = bar_base + 8 * STAGES;
-  const uint32_t tfull_bar = bar_base + 16 * STAGES, tempty_bar = tfull_bar + 16;
-  uint8_t* smem_al = smem_raw + (smem_base - smem_u32(smem_raw));
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(smem_al + (bar_base - smem_base) + 16 * STAGES + 32);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int num_kb = (p.K + BK - 1) / BK;
-  const int num_chunks = (num_kb + CHUNK_KB - 1) / CHUNK_KB;
-  // persistent tile loop: pair `pair` takes tiles pair, pair + num_pairs, ...; n fastest, so the pairs running concurrently cover all
-  // n-tiles of a few m-tiles: each A panel is fetched from HBM once and the (small) B operand stays L2-resident
-  const int tiles_m = (p.M + 255) / 256, tiles_n = (p.N + BN - 1) / BN;
-  const long long total_tiles = (long long)tiles_m * tiles_n * p.nbx * p.nby;
-  const int pair = blockIdx.x >> 1, num_pairs = gridDim.x >> 1;
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(tfull_bar + 8 * b, 1); mbar_init(tempty_bar + 8 * b, 2 * EW); }  // EW epilogue warps x 2 CTAs
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"((uint32_t)(2 * BN)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-
-  if (warp == 0) {
-    if (elect_one_sync()) {   // one lane, known to ptxas: uniform-datapath issue without per-instruction waterfall loops
-      const int cblk = (p.a_mode == 1) ? p.cv_cin / BK : 0;
-      const uint32_t leader_full = full_bar & 0xFEFFFFFFu;   // same offset in the even (leader) CTA of the pair
-      long long g = 0;                                        // global k-block counter (stage ring position)
-      for (long long tile = pair; tile < total_tiles; tile += num_pairs) {
-        const int nt = (int)(tile % tiles_n);
-        const int mt = (int)((tile / tiles_n) % tiles_m);
-        const int z = (int)(tile / ((long long)tiles_m * tiles_n));
-        if (band_skip(p.band_t, mt * 256, 256, nt * BN, BN)) continue;
-        const int bx = z % p.nbx, by = z / p.nbx;
-        const int m0 = mt * 256 + (int)rank * 128, nb = nt * BN + (int)rank * BH;
-        for (int kb = 0; kb < num_kb; ++kb, ++g) {
-          const int s = (int)(g % STAGES);
-          const uint32_t ph = (uint32_t)((g / STAGES) & 1);
-          mbar_wait(empty_bar + 8 * s, ph ^ 1);
-          if (leader) mbar_expect_tx(full_bar + 8 * s, 2 * STAGE_BYTES);  // bytes of both CTAs land on the leader's barrier
-          const uint32_t fb = leader_full + 8 * s;
-          const uint32_t sa = smem_base + s * STAGE_BYTES;
-          if (p.a_mode == 0) {
-            const int ko = (p.kob > 0) ? kb / p.kob : 0;
-            const int ki = (p.kob > 0) ? kb % p.kob : kb;
-            tma_load_5d_2sm(sa, &tmA, fb, ki * BK, m0, bx * axm + ko, by * aym, 0);
-            tma_load_5d_2sm(sa + A_TILE_BYTES, &tmA, fb, ki * BK, m0, bx * axm + ko, by * aym, 1);
-          } else {
-            const int tap = kb / cblk, c0 = (kb % cblk) * BK;
-            const int kt = tap / 3, kf = tap % 3;
-            const int par = (kt & 1) * 2 + (kf & 1);
-            tma_load_5d_2sm(sa, &tmA, fb, c0, m0 + (kt >> 1), bx + (kf >> 1), par, by);
-            tma_load_5d_2sm(sa + A_TILE_BYTES, &tmA, fb, c0, m0 + (kt >> 1), bx + (kf >> 1), 4 + par, by);
-          }
-          tma_load_5d_2sm(sa + 2 * A_TILE_BYTES, &tmB, fb, kb * BK, nb, bx * bxm, by * bym, 0);
-          tma_load_5d_2sm(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, &tmB, fb, kb * BK, nb, bx * bxm, by * bym, 1);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (leader && elect_one_sync()) {
-      const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-      long long g = 0, cg = 0;                                // global k-block / chunk counters
-      for (long long tile = pair; tile < total_tiles; tile += num_pairs) {
-        if (band_skip(p.band_t, (int)((tile / tiles_n) % tiles_m) * 256, 256, (int)(tile % tiles_n) * BN, BN)) continue;
-        for (int c = 0; c < num_chunks; ++c, ++cg) {
-          const int b = (int)(cg & 1);
-          mbar_wait(tempty_bar + 8 * b, (uint32_t)(((cg >> 1) & 1) ^ 1));   // both CTAs' epilogues have drained this accumulator buffer
-          tcgen05_fence_after();
-          const uint32_t d = tmem_base + (uint32_t)(b * BN);
-          const int kb_end = min(num_kb, (c + 1) * CHUNK_KB);
-          for (int kb = c * CHUNK_KB; kb < kb_end; ++kb, ++g) {
-            const int s = (int)(g % STAGES);
-            const uint32_t ph = (uint32_t)((g / STAGES) & 1);
-            mbar_wait(full_bar + 8 * s, ph);
-            tcgen05_fence_after();
-            const uint32_t sa = smem_base + s * STAGE_BYTES;
-#pragma unroll
-            for (int k = 0; k < BK / 8; ++k) {
-              const uint64_t a_hi = umma_desc(sa + k * 32), a_lo = umma_desc(sa + A_TILE_BYTES + k * 32);
-              const uint64_t b_hi = umma_desc(sa + 2 * A_TILE_BYTES + k * 32);
-              const uint64_t b_lo = umma_desc(sa + 2 * A_TILE_BYTES + B_TILE_BYTES + k * 32);
-              mma_tf32_2sm(d, a_lo, b_hi, idesc, (kb != c * CHUNK_KB || k != 0) ? 1u : 0u);
-              mma_tf32_2sm(d, a_hi, b_lo, idesc, 1);
-              mma_tf32_2sm(d, a_hi, b_hi, idesc, 1);
-            }
-            tcgen05_commit_2sm(empty_bar + 8 * s);
-          }
-          tcgen05_commit_2sm(tfull_bar + 8 * b);
-        }
-      }
-    }
-  } else {
-    const int e = warp - 2, q = warp & 3, half = e >> 2;   // a warp may only touch TMEM lanes 32*(warp_id%4)..+31
-    float* xp = reinterpret_cast<float*>(smem_al + (xp_base - smem_base)) + e * XP_FLOATS;
-    long long cg = 0;
-    for (long long tile = pair; tile < total_tiles; tile += num_pairs) {
-      const int nt = (int)(tile % tiles_n);
-      const int mt = (int)((tile / tiles_n) % tiles_m);
-      const int z = (int)(tile / ((long long)tiles_m * tiles_n));
-      if (band_skip(p.band_t, mt * 256, 256, nt * BN, BN)) continue;
-      const int bx = z % p.nbx, by = z / p.nbx;
-      const int m0 = mt * 256 + (int)rank * 128, n0 = nt * BN;
-      float acc[CW];
-#pragma unroll
-      for (int j = 0; j < CW; ++j) acc[j] = 0.f;
-      for (int c = 0; c < num_chunks; ++c, ++cg) {
-        const int b = (int)(cg & 1);
-        mbar_wait(tfull_bar + 8 * b, (uint32_t)((cg >> 1) & 1));
-        tcgen05_fence_after();
-#pragma unroll
-        for (int j = 0; j < CW / LDW; ++j) {
-          float v[LDW];
-          __syncwarp();
-          const uint32_t ta = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(b * BN + half * CW + j * LDW);
-          if (LDW == 32) tmem_ld32(ta, v); else tmem_ld16(ta, v);
-#pragma unroll
-          for (int i = 0; i < LDW; ++i) acc[j * LDW + i] += v[i];
-        }
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_remote(tempty_bar + 8 * b, 0);   // leader CTA's barrier (local or remote)
-      }
-      // ---- epilogue: 32x32 blocks are transposed through smem (two 16-row halves) so that every global access of a warp covers four
-      // 128-byte row segments with 128-bit accesses; residual and bias values are fetched before the math so that loads overlap.
-      EpiArgs ea;
-      const long long coff = (long long)by * p.sc_y + (long long)bx * p.sc_x;
-      const long long roff = (long long)by * p.sr_y + (long long)bx * p.sr_x;
-      ea.C = p.C + coff; ea.c_plane = p.c_plane; ea.ldc = p.ldc; ea.split_out = p.split_out;
-      ea.bias = p.bias ? p.bias + (long long)bx * p.sbias_x : nullptr; ea.R = p.R ? p.R + roff : nullptr;
-      ea.ldr = p.ldr; ea.alpha = p.alpha; ea.act = p.act;
-      const bool vec_ok = ((p.ldc & 3) == 0) && ((coff & 3) == 0) && ((p.c_plane & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0) &&
-                          (!p.R || (((p.ldr & 3) == 0) && ((roff & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.R) & 15) == 0))) &&
-                          (!p.bias || ((((long long)bx * p.sbias_x) & 3) == 0 && (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0));
-      const int row0 = m0 + q * 32;
-      const int rsub = lane >> 3, c4 = (lane & 7) * 4;     // read mapping: 4 rows x 8 float4 per warp access
-      const int rows_left = p.M - row0 - rsub;             // this lane's rows row0 + rsub + 4k are valid while 4k < rows_left
-      const long long ldc = ea.ldc, ldr = ea.ldr, cpl = ea.c_plane;
-      const int Ncols = p.N;
-      const float alpha = ea.alpha;
-      const bool has_r = ea.R != nullptr;
-      float* const crow0 = ea.C + (long long)(row0 + rsub) * ldc;
-      const float* const rrow0 = has_r ? ea.R + (long long)(row0 + rsub) * ldr : nullptr;
-      float* const wrow = xp + (lane & (XR - 1)) * 36;
-      const float* const rbase = xp + rsub * 36 + c4;
-      // 128-bit path: row / column predicates only (warp-uniform block skips), pointers advanced incrementally
-      if (vec_ok) {
-        const bool has_b = ea.bias != nullptr;
-#pragma unroll
-        for (int j = 0; j < CW / 32; ++j) {
-          const int colb = n0 + half * CW + j * 32;
-          if (row0 >= p.M || colb >= Ncols) continue;          // warp-uniform: block entirely outside the matrix
-          if (c_band_blocks && band_skip(p.band_t, row0, 32, colb, 32)) continue;  // rel-pos band product: a 32 x 32 block no (query, key) pair reaches is not stored
-          if (PLAIN && row0 + 32 <= p.M && colb + 32 <= Ncols) {
-            // interior block of a product without bias / residual / scaling (attention scores, context): straight-line transpose + stores,
-            // no per-row or per-column predicates (the generic path below spends most of its issue slots on them)
-#pragma unroll
-            for (int hh = 0; hh < NH; ++hh) {
-              __syncwarp();
-              if ((lane / XR) == hh) {
-#pragma unroll
-                for (int i = 0; i < 32; i += 4)
-                  *reinterpret_cast<float4*>(wrow + i) = make_float4(acc[j * 32 + i], acc[j * 32 + i + 1], acc[j * 32 + i + 2], acc[j * 32 + i + 3]);
-              }
-              __syncwarp();
-              float* cpi = crow0 + (long long)(hh * XR) * ldc + colb + c4;
-#pragma unroll 2
-              for (int it = 0; it < ITS; ++it, cpi += 4 * ldc) {
-                const float4 v = *reinterpret_cast<const float4*>(rbase + it * 4 * 36);
-                if (SPLIT) {
-                  float4 h, l;
-                  h.x = espb::tf32_hi(v.x); h.y = espb::tf32_hi(v.y); h.z = espb::tf32_hi(v.z); h.w = espb::tf32_hi(v.w);
-                  l.x = espb::tf32_lo(v.x, h.x); l.y = espb::tf32_lo(v.y, h.y); l.z = espb::tf32_lo(v.z, h.z); l.w = espb::tf32_lo(v.w, h.w);
-                  *reinterpret_cast<float4*>(cpi) = h;
-                  *reinterpret_cast<float4*>(cpi + cpl) = l;
-                } else {
-                  *reinterpret_cast<float4*>(cpi) = v;
-                }
-              }
-            }
-            continue;
-          }
-          const int col = colb + c4;
-          const bool c_full = col + 3 < Ncols, c_part = !c_full && col < Ncols;
-          float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (!PLAIN && has_b && c_full) b4 = __ldg(reinterpret_cast<const float4*>(ea.bias + col));
-#pragma unroll
-          for (int hh = 0; hh < NH; ++hh) {
-            __syncwarp();
-            if ((lane / XR) == hh) {
-#pragma unroll
-              for (int i = 0; i < 32; i += 4)
-                *reinterpret_cast<float4*>(wrow + i) = make_float4(acc[j * 32 + i], acc[j * 32 + i + 1], acc[j * 32 + i + 2], acc[j * 32 + i + 3]);
-            }
-            __syncwarp();
-            float* cp = crow0 + (long long)(hh * XR) * ldc + col;
-            float4 rv[ITS];
-#pragma unroll
-            for (int it = 0; it < ITS; ++it) {
-              rv[it] = make_float4(0.f, 0.f, 0.f, 0.f);
-              if (!PLAIN && has_r && c_full && hh * XR + it * 4 < rows_left)
-                rv[it] = *reinterpret_cast<const float4*>(rrow0 + (long long)(hh * XR + it * 4) * ldr + col);
-            }
-#pragma unroll
-            for (int it = 0; it < ITS; ++it) {
-              const int rl = hh * XR + it * 4;
-              if (rl >= rows_left) continue;
-              const float4 v = *reinterpret_cast<const float4*>(rbase + it * 4 * 36);
-              float* cpi = cp + (long long)(it * 4) * ldc;
-              if (c_full) {
-                float t[4] = {v.x, v.y, v.z, v.w};
-                if (!PLAIN) {
-                  const float bb4[4] = {b4.x, b4.y, b4.z, b4.w};
-                  const float rr4[4] = {rv[it].x, rv[it].y, rv[it].z, rv[it].w};
-#pragma unroll
-                  for (int i = 0; i < 4; ++i) {
-                    float x = t[i] + bb4[i];
-                    if (ACT == espb::ACT_RELU) x = fmaxf(x, 0.f);
-                    else if (ACT == espb::ACT_SWISH) x = __fdividef(x, 1.f + __expf(-x));
-                    t[i] = fmaf(alpha, x, rr4[i]);
-                  }
-                }
-                if (SPLIT) {
-                  float4 h, l;
-                  h.x = espb::tf32_hi(t[0]); h.y = espb::tf32_hi(t[1]); h.z = espb::tf32_hi(t[2]); h.w = espb::tf32_hi(t[3]);
-                  l.x = espb::tf32_lo(t[0], h.x); l.y = espb::tf32_lo(t[1], h.y); l.z = espb::tf32_lo(t[2], h.z); l.w = espb::tf32_lo(t[3], h.w);
-                  *reinterpret_cast<float4*>(cpi) = h;
-                  *reinterpret_cast<float4*>(cpi + cpl) = l;
-                } else {
-                  *reinterpret_cast<float4*>(cpi) = make_float4(t[0], t[1], t[2], t[3]);
-                }
-              } else if (c_part) {   // the one float4 per row that straddles N
-                const float vv[4] = {v.x, v.y, v.z, v.w};
-                for (int i = 0; i < 4 && col + i < Ncols; ++i) {
-                  const float tt = epi_value(ea, vv[i], row0 + rsub + rl, col + i);
-                  if (SPLIT) { const float hh2 = espb::tf32_hi(tt); cpi[i] = hh2; cpi[cpl + i] = espb::tf32_lo(tt, hh2); }
-                  else cpi[i] = tt;
-                }
-              }
-            }
-          }
-        }
-      } else {
-        // unaligned output / residual / bias (never on the hot path): scalar stores
-#pragma unroll 1
-        for (int j = 0; j < CW / 32; ++j) {
-          const int colb = n0 + half * CW + j * 32;
-          if (row0 >= p.M || colb >= Ncols) continue;
-          if (c_band_blocks && band_skip(p.band_t, row0, 32, colb, 32)) continue;
-#pragma unroll 1
-          for (int hh = 0; hh < NH; ++hh) {
-            __syncwarp();
-            if ((lane / XR) == hh) {
-              for (int i = 0; i < 32; ++i) wrow[i] = acc_at(acc, j * 32 + i);
-            }
-            __syncwarp();
-            for (int it = 0; it < ITS; ++it) {
-              const int rl = hh * XR + it * 4;
-              if (rl >= rows_left) continue;
-              for (int i = 0; i < 4; ++i) {
-                const int col = colb + c4 + i;
-                if (col < Ncols) {
-                  const long long row = row0 + rsub + rl;
-                  const float tt = epi_value(ea, rbase[it * 4 * 36 + i], row, col);
-                  float* cpe = ea.C + row * ldc + col;
-                  if (SPLIT) { const float hh2 = espb::tf32_hi(tt); cpe[0] = hh2; cpe[cpl] = espb::tf32_lo(tt, hh2); }
-                  else cpe[0] = tt;
-                }
-              }
-            }
-          }
-        }
-      }
-    }
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  cluster_sync_all();   // the peer may still read this CTA's smem / signal its barriers until both are done
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)(2 * BN)) : "memory");
+  for (int j = 0; j < BN / 8; ++j) {
+    const float* r = PROMOTE ? acc : part;
+    epi_store2(e, row, col + 8 * j, r[4 * j], r[4 * j + 1], p.M, p.N, vec_ok);
+    epi_store2(e, row + 8, col + 8 * j, r[4 * j + 2], r[4 * j + 3], p.M, p.N, vec_ok);
   }
 }
 
@@ -882,125 +258,35 @@ int make_map(CUtensorMap* map, const float* base, const long long dims[5], const
   return espb_make_tensor_map(map, base, dims, strides_el, BK, box_rows, 1);
 }
 
-template <int BN, int STAGES>
+template <int BN, int STAGES, bool PROMOTE>
 int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const EspbGemmDesc& d, int bxm, int bym, int axm, int aym, cudaStream_t stream) {
-  constexpr int smem = STAGES * (2 * A_TILE_BYTES + 2 * BN * 128) + 1024 + 16 * STAGES + 16;
-  static bool attr_set = false;
-  if (!attr_set) {
-    if (cudaFuncSetAttribute(gemm_tf32x3_kernel<BN, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
-      espb_set_error("cudaFuncSetAttribute(max dynamic smem) failed");
-      return ESPB_ERR_CUDA;
-    }
-    attr_set = true;
-  }
-  dim3 grid((d.M + BM - 1) / BM, (d.N + BN - 1) / BN, d.nbx * d.nby);
-  if (espb::launch_pdl(gemm_tf32x3_kernel<BN, STAGES>, grid, dim3(NUM_THREADS), smem, stream, tmA, tmB, d, bxm, bym, axm, aym) != cudaSuccess) {
-    espb_set_error(cudaGetErrorString(cudaGetLastError())); return ESPB_ERR_CUDA;
-  }
-  return ESPB_OK;
-}
-
-template <int BN, int STAGES, int ACT, bool SPLIT, bool PLAIN, int EW>
-int launch_tc2_ew(const CUtensorMap& tmA, const CUtensorMap& tmB, const EspbGemmDesc& d, int bxm, int bym, int axm, int aym, cudaStream_t stream) {
-  constexpr int smem = STAGES * (2 * A_TILE_BYTES + 2 * (BN / 2) * 128) + 128 * 36 * 4 + 1024 + 16 * STAGES + 64;
+  constexpr int smem = STAGES * (2 * A_TILE_BYTES + 2 * BN * 128) + 1024 + 16 * STAGES;
   static_assert(smem <= 232448, "dynamic shared memory budget exceeded");
   static bool attr_set = false;
-  static int num_sms = 0;
   if (!attr_set) {
-    if (cudaFuncSetAttribute(gemm_tf32x3_2cta_kernel<BN, STAGES, ACT, SPLIT, PLAIN, EW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
-      espb_set_error("cudaFuncSetAttribute(max dynamic smem) failed");
-      return ESPB_ERR_CUDA;
-    }
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (getenv("ESPB_GEMM_BAND_TILES_ONLY")) { const int zero = 0; cudaMemcpyToSymbol(c_band_blocks, &zero, sizeof(int)); }
-    attr_set = true;
-  }
-  const long long tiles = (long long)((d.M + 255) / 256) * ((d.N + BN - 1) / BN) * d.nbx * d.nby;
-  const long long pairs = tiles < num_sms / 2 ? tiles : num_sms / 2;   // persistent: one CTA pair per SM pair
-  dim3 grid((unsigned)(2 * pairs), 1, 1);
-  gemm_tf32x3_2cta_kernel<BN, STAGES, ACT, SPLIT, PLAIN, EW><<<grid, 64 + 32 * EW, smem, stream>>>(tmA, tmB, d, bxm, bym, axm, aym);
-  ESPB_CHECK_LAUNCH();
-  return ESPB_OK;
-}
-
-// 256 accumulator columns with a hi / lo split output: 16 epilogue warps x 64 columns (half the accumulator registers per thread, twice the
-// warps to hide the latency of the activation / split / two-plane store chain).  Measured at M 59968 (scripts/gemm_enc_microbench.py): FFN w_1
-// (Swish, split) 653 -> 588 us, plain split N 512 215 -> 168 us; the single-plane epilogues are store-light and 2-3 % faster with 8 warps, so
-// they keep them.  ESPB_GEMM_EW8=1 forces the 8-warp epilogue everywhere (A/B measurements).
-template <int BN, int STAGES, int ACT, bool SPLIT, bool PLAIN>
-int launch_tc2_v(const CUtensorMap& tmA, const CUtensorMap& tmB, const EspbGemmDesc& d, int bxm, int bym, int axm, int aym, cudaStream_t stream) {
-  if (BN >= 256 && SPLIT) {
-    static int ew8 = -1;
-    if (ew8 < 0) ew8 = getenv("ESPB_GEMM_EW8") ? 1 : 0;
-    if (!ew8) return launch_tc2_ew<BN, STAGES, ACT, SPLIT, PLAIN, (BN >= 256 && SPLIT) ? 16 : 8>(tmA, tmB, d, bxm, bym, axm, aym, stream);
-  }
-  return launch_tc2_ew<BN, STAGES, ACT, SPLIT, PLAIN, 8>(tmA, tmB, d, bxm, bym, axm, aym, stream);
-}
-
-template <int BN, int STAGES>
-int launch_tc2(const CUtensorMap& tmA, const CUtensorMap& tmB, const EspbGemmDesc& d, int bxm, int bym, int axm, int aym, cudaStream_t stream) {
-  const int v = d.act * 2 + (d.split_out ? 1 : 0);
-  const bool plain = d.act == espb::ACT_NONE && d.bias == nullptr && d.R == nullptr && d.alpha == 1.0f && !getenv("ESPB_GEMM_NO_PLAIN");
-  if (plain) {
-    if (d.split_out) return launch_tc2_v<BN, STAGES, espb::ACT_NONE, true, true>(tmA, tmB, d, bxm, bym, axm, aym, stream);
-    return launch_tc2_v<BN, STAGES, espb::ACT_NONE, false, true>(tmA, tmB, d, bxm, bym, axm, aym, stream);
-  }
-  switch (v) {
-    case 0: return launch_tc2_v<BN, STAGES, espb::ACT_NONE, false, false>(tmA, tmB, d, bxm, bym, axm, aym, stream);
-    case 1: return launch_tc2_v<BN, STAGES, espb::ACT_NONE, true, false>(tmA, tmB, d, bxm, bym, axm, aym, stream);
-    case 2: return launch_tc2_v<BN, STAGES, espb::ACT_RELU, false, false>(tmA, tmB, d, bxm, bym, axm, aym, stream);
-    case 3: return launch_tc2_v<BN, STAGES, espb::ACT_RELU, true, false>(tmA, tmB, d, bxm, bym, axm, aym, stream);
-    case 4: return launch_tc2_v<BN, STAGES, espb::ACT_SWISH, false, false>(tmA, tmB, d, bxm, bym, axm, aym, stream);
-    case 5: return launch_tc2_v<BN, STAGES, espb::ACT_SWISH, true, false>(tmA, tmB, d, bxm, bym, axm, aym, stream);
-    default: espb_set_error("gemm: unknown activation"); return ESPB_ERR_ARG;
-  }
-}
-
-template <int BN, int STAGES, int MC>
-int launch_tc_mc(const CUtensorMap& tmA, const CUtensorMap& tmB, const EspbGemmDesc& d, int bxm, int bym, int axm, int aym, cudaStream_t stream) {
-  constexpr int smem = STAGES * (2 * A_TILE_BYTES + 2 * BN * 128) + 1024 + 16 * STAGES + 16;
-  static bool attr_set = false;
-  if (!attr_set) {
-    if (cudaFuncSetAttribute(gemm_tf32x3_mc_kernel<BN, STAGES, MC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
+    if (cudaFuncSetAttribute(gemm_tf32x3_kernel<BN, STAGES, PROMOTE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
       espb_set_error("cudaFuncSetAttribute(max dynamic smem) failed");
       return ESPB_ERR_CUDA;
     }
     attr_set = true;
   }
   dim3 grid((d.M + BM - 1) / BM, (d.N + BN - 1) / BN, d.nbx * d.nby);
-  if (espb::launch_pdl(gemm_tf32x3_mc_kernel<BN, STAGES, MC>, grid, dim3(NUM_THREADS), smem, stream, tmA, tmB, d, bxm, bym, axm, aym) != cudaSuccess) {
+  if (espb::launch_pdl(gemm_tf32x3_kernel<BN, STAGES, PROMOTE>, grid, dim3(NUM_THREADS), smem, stream, tmA, tmB, d, bxm, bym, axm, aym) != cudaSuccess) {
     espb_set_error(cudaGetErrorString(cudaGetLastError())); return ESPB_ERR_CUDA;
   }
   return ESPB_OK;
 }
 
-template <int BN, int STAGES, int SK>
-int launch_tc_sk(const CUtensorMap& tmA, const CUtensorMap& tmB, const EspbGemmDesc& d, cudaStream_t stream) {
-  constexpr int smem = STAGES * (2 * A_TILE_BYTES + 2 * BN * 128) + 1024 + 16 * STAGES + 16;
-  static bool attr_set = false;
-  if (!attr_set) {
-    if (cudaFuncSetAttribute(gemm_tf32x3_sk_kernel<BN, STAGES, SK>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
-      espb_set_error("cudaFuncSetAttribute(max dynamic smem) failed");
-      return ESPB_ERR_CUDA;
-    }
-    attr_set = true;
+int num_sms() {
+  static int n = 0;
+  if (n == 0) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    if (n <= 0) n = 1;
   }
-  dim3 grid((d.M + BM - 1) / BM, (d.N + BN - 1) / BN, SK);
-  if (espb::launch_pdl(gemm_tf32x3_sk_kernel<BN, STAGES, SK>, grid, dim3(NUM_THREADS), smem, stream, tmA, tmB, d) != cudaSuccess) {
-    espb_set_error(cudaGetErrorString(cudaGetLastError())); return ESPB_ERR_CUDA;
-  }
-  return ESPB_OK;
+  return n;
 }
-
-// ESPB_GEMM_SPLITK=0 disables the split-K decode kernels (A/B measurements); read once.
-bool splitk_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("ESPB_GEMM_SPLITK"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v == 1;
-}
-
 }  // namespace
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -1077,62 +363,20 @@ int espb_gemm_tc_launch(const EspbGemmDesc& d, cudaStream_t stream, int version)
   if (rc != ESPB_OK) return rc;
   const int bxm = d.sb_x != 0 ? 1 : 0, bym = d.sb_y != 0 ? 1 : 0;
   const long long tiles_m = (d.M + BM - 1) / BM, nb = (long long)d.nbx * d.nby;
-  if (version == 2 && (long long)d.M * d.nbx * d.nby > 1024) {   // tiny (decode-step) problems are latency-bound: 128x64 1-CTA tiles spread them over more SMs
-    // CTA-pair kernel: 256 x BN tiles; B box = BN/2 rows per CTA
-    const int bn = (d.N <= 64 && !getenv("ESPB_GEMM_NO_BN64")) ? 64 : (d.N <= 128) ? 128 : 256;   // N = d_k products (p.v, decoder memory K/V) waste no MMA columns
-    long long dims[5] = {d.K, d.N, bxm ? d.nbx : 1, bym ? d.nby : 1, 2};
-    long long str[4] = {d.ldb, d.sb_x, d.sb_y, d.b_plane};
-    rc = make_map(&tmB, d.B, dims, str, bn / 2);
-    if (rc != ESPB_OK) return rc;
-    if (bn == 256) return launch_tc2<256, 3>(tmA, tmB, d, bxm, bym, axm, aym, stream);
-    if (bn == 64) return launch_tc2<64, 5>(tmA, tmB, d, bxm, bym, axm, aym, stream);
-    return launch_tc2<128, 4>(tmA, tmB, d, bxm, bym, axm, aym, stream);
-  }
-  if (version == 2 && nb == 1 && d.a_mode == 0 && d.band_t == 0 && d.kob == 0 && d.N > 64 && splitk_enabled()) {
-    // decode-step shapes: split K over a cluster while the whole problem still fits one wave of 1-CTA tiles
-    const long long tiles128 = tiles_m * ((d.N + 127) / 128);
-    const int num_kb = (d.K + BK - 1) / BK;
-    int sk = 0;
-    auto all_ranks_busy = [&](int n) { return (n - 1) * ((num_kb + n - 1) / n) < num_kb; };   // every K slice holds >= 1 k-block
-    if (tiles128 * 4 <= 148 && num_kb >= 8 && all_ranks_busy(4)) sk = 4;
-    else if (tiles128 * 2 <= 148 && num_kb >= 4 && all_ranks_busy(2)) sk = 2;
-    if (sk) {
-      long long dims[5] = {d.K, d.N, 1, 1, 2};
-      long long str[4] = {d.ldb, 0, 0, d.b_plane};
-      rc = make_map(&tmB, d.B, dims, str, 128);
-      if (rc != ESPB_OK) return rc;
-      if (sk == 4) return launch_tc_sk<128, 3, 4>(tmA, tmB, d, stream);
-      return launch_tc_sk<128, 3, 2>(tmA, tmB, d, stream);
-    }
-  }
-  int bn;
-  if (d.N <= 64) bn = 64;
-  else if (d.N <= 128) bn = 128;
-  else if (tiles_m * ((d.N + 255) / 256) * nb >= 148) bn = 256;
-  else if (tiles_m * ((d.N + 127) / 128) * nb >= 148) bn = 128;
-  else if (tiles_m * ((d.N + 63) / 64) * nb > 148) bn = 128;   // one CTA per SM (192 KB smem): more than 148 tiles would run as two waves
-  else bn = 64;
+  // 128-column tiles unless the problem then has fewer tiles than SMs (decode-step shapes): 64-column tiles spread it over more SMs
+  const int bn = (d.N <= 64 || tiles_m * ((d.N + 127) / 128) * nb < num_sms()) ? 64 : 128;
   {
     long long dims[5] = {d.K, d.N, bxm ? d.nbx : 1, bym ? d.nby : 1, 2};
     long long str[4] = {d.ldb, d.sb_x, d.sb_y, d.b_plane};
     rc = make_map(&tmB, d.B, dims, str, bn);
     if (rc != ESPB_OK) return rc;
   }
-  if (bn == 256) return launch_tc<256, 2>(tmA, tmB, d, bxm, bym, axm, aym, stream);
-  const bool mc_ok = version == 2 && d.a_mode == 0 && d.band_t == 0 && ((d.N + bn - 1) / bn) % 4 == 0 && bn <= 128;
-  if (mc_ok) {
-    // decode-step problems: 4 neighbouring n-tiles share (multicast) the A tile; A box = 32 rows per CTA
-    long long n_outer = 1, k_inner = d.K;
-    if (d.kob > 0) { k_inner = (long long)d.kob * BK; n_outer = (d.K + k_inner - 1) / k_inner; }
-    long long dims[5] = {k_inner, d.M, (axm ? d.nbx : 1) + n_outer - 1, aym ? d.nby : 1, 2};
-    long long str[4] = {d.lda, d.sa_x, d.sa_y, d.a_plane};
-    rc = make_map(&tmA, d.A, dims, str, BM / 4);
-    if (rc != ESPB_OK) return rc;
-    if (bn == 128) return launch_tc_mc<128, 3, 4>(tmA, tmB, d, bxm, bym, axm, aym, stream);
-    return launch_tc_mc<64, 4, 4>(tmA, tmB, d, bxm, bym, axm, aym, stream);
+  if (version == 2) {
+    if (bn == 128) return launch_tc<128, 3, true>(tmA, tmB, d, bxm, bym, axm, aym, stream);
+    return launch_tc<64, 4, true>(tmA, tmB, d, bxm, bym, axm, aym, stream);
   }
-  if (bn == 128) return launch_tc<128, 3>(tmA, tmB, d, bxm, bym, axm, aym, stream);
-  return launch_tc<64, 4>(tmA, tmB, d, bxm, bym, axm, aym, stream);
+  if (bn == 128) return launch_tc<128, 3, false>(tmA, tmB, d, bxm, bym, axm, aym, stream);
+  return launch_tc<64, 4, false>(tmA, tmB, d, bxm, bym, axm, aym, stream);
 }
 
 int espb_gemm_simt_launch(const EspbGemmDesc& d, cudaStream_t stream) {

@@ -1,10 +1,10 @@
-// GEMM descriptor shared by the tcgen05 3xTF32 kernel and the SIMT fp32 kernel.
+// GEMM descriptor shared by the wgmma 3xTF32 kernel and the SIMT fp32 kernel.
 //
 //   C[by,bx][m, n] = epilogue( sum_k A[by,bx][m, k] * B[by*bym, bx*bxm][n, k] )
 //
 // A and B are "split" fp32 tensors: two planes (hi, lo) `*_plane` elements apart, produced by
 // espb::tf32_hi/tf32_lo; the tensor-core kernel forms A_lo*B_hi + A_hi*B_lo + A_hi*B_hi in
-// fp32 TMEM accumulators (error-compensated 3xTF32, ~2^-21 relative per product); the SIMT
+// fp32 register accumulators (error-compensated 3xTF32, ~2^-21 relative per product); the SIMT
 // kernel adds the planes back (hi+lo is the original fp32 value up to 2^-22) and uses FFMA.
 // Both operands are K-major (row-major [rows, K]).
 #pragma once
@@ -28,5 +28,5 @@ struct EspbGemmDesc {
   int band_t;           // > 0: only columns n with band_t-1-m <= n <= 2*band_t-2-m are ever read (rel-pos shift): tiles outside are skipped
 };
 
-int espb_gemm_tc_launch(const EspbGemmDesc& d, cudaStream_t stream, int version);  // tcgen05 (1: 1-CTA, 2: CTA pair + chunked promotion)
+int espb_gemm_tc_launch(const EspbGemmDesc& d, cudaStream_t stream, int version);  // wgmma (1: plain accumulation, 2: chunked promotion)
 int espb_gemm_simt_launch(const EspbGemmDesc& d, cudaStream_t stream);  // any strides

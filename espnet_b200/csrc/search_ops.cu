@@ -1163,8 +1163,8 @@ int espb_dec_src_attn_f32(const float* q, const float* kmem, const float* vmem, 
     if (dk == 64 && !getenv("ESPNET_B200_SRC_ATTN_FFMA") && !getenv("ESPNET_B200_SRC_ATTN_TWOPASS")) {
       // single-pass kernel: 3 stages of (K, V) tiles = 112 KB -> two blocks per SM, 128 KB of loads in flight per SM
       using FlashFn = void (*)(const float*, const float*, const float*, int, const int*, int, int, int, float*, long long, int, int);
-      // NW = 4 (default): four 57 KB blocks per SM, 592 resident -- a 64-utterance x 8-head launch is one wave; NW = 8 (ESPB_SRC_ATTN_NW=8, the
-      // first version): two 112 KB blocks per SM, 296 resident = 1.73 waves.  Same bytes in flight per SM; measured 80.9 -> 74.9 us per launch.
+      // NW = 4 (default): four 57 KB blocks per SM -- 528 resident on an H100's 132 SMs, so a 64-utterance x 8-head launch is one wave; NW = 8
+      // (ESPB_SRC_ATTN_NW=8, the first version): two 112 KB blocks per SM.  Same bytes in flight per SM.
       static int nw = 0;
       if (!nw) { const char* e = getenv("ESPB_SRC_ATTN_NW"); nw = (e && e[0] == '8') ? 8 : (e && e[0] == '4') ? 4 : ESPB_SRC_ATTN_NW_DEFAULT; }
       const FlashFn fn = (nw == 4) ? dec_src_attn_flash_kernel<3, 4> : dec_src_attn_flash_kernel<3, 8>;

@@ -1,5 +1,5 @@
 """ConformerEncoder with the reference's constructor / state_dict surface, executed by the espnet_b200
-CUDA kernels (tcgen05 3xTF32 GEMMs + warp-primitive glue).
+CUDA kernels (wgmma 3xTF32 GEMMs + warp-primitive glue).
 
 Reference: espnet2/asr/encoder/conformer_encoder.py:89-429 and the legacy modules it composes
 (Conv2dSubsampling, RelPositionalEncoding, EncoderLayer, RelPositionMultiHeadedAttention,
@@ -259,7 +259,7 @@ class ConformerEncoder(torch.nn.Module):
         qu, qv = self._buf("qu", (2, M, D)), self._buf("qv", (2, M, D))
         vt = self._buf("vt", (2, B, H, dk, Tp))
         bd = self._buf("bd", (B, H, T, Rp))
-        fused = ops.use_flash_attn(dk)      # one tcgen05 kernel for q k^T + rel_shift + softmax + p v (csrc/attention.cu); else materialised
+        fused = ops.use_flash_attn(dk)      # one wgmma kernel for q k^T + rel_shift + softmax + p v (csrc/attention.cu); else materialised
         if not fused:
             ac = self._buf("ac", (B, H, T, Tp))
             probs = self._buf("probs", (2, B, H, T, Tp))

@@ -12,7 +12,7 @@ from .lib import GemmDesc, call, ptr
 
 ACT_NONE, ACT_RELU, ACT_SWISH = 0, 1, 2
 
-# GEMM kernel: "tc" = tcgen05 1-CTA, "tc2" = tcgen05 CTA pair + chunked fp32 promotion, "simt" = FFMA (bring-up / A-B checks);
+# GEMM kernel: "tc" = wgmma 3xTF32, "tc2" = wgmma 3xTF32 with chunked fp32 promotion, "simt" = FFMA (bring-up / A-B checks);
 # shapes TMA cannot address always use SIMT.
 _GEMM_MODE = os.environ.get("ESPNET_B200_GEMM", "tc2")
 launch_counter = [0]
@@ -87,7 +87,7 @@ def gemm(M, N, K, A, a_plane, lda, B, b_plane, ldb, C, ldc, *, c_plane=0, split_
     if prof is not None:
         e1.record()
         n_alg = band_t if band_t > 0 else N     # rel-pos band product: every row needs band_t of the N columns
-        prof.append((2.0 * M * n_alg * K * nbx * nby, e0, e1, use_tc == 2 and M * nbx * nby > 1024))   # last: CTA-pair kernel?
+        prof.append((2.0 * M * n_alg * K * nbx * nby, e0, e1))
     _count()
     return bool(use_tc)
 
@@ -101,7 +101,7 @@ def linear(x_split, w_split, out, *, bias=None, act=ACT_NONE, residual=None, alp
                 R=residual, ldr=N, alpha=alpha, act=act, force=force)
 
 
-# Fused tcgen05 self-attention (csrc/attention.cu) for d_k = 64; ESPB_ATTN=materialized keeps the round-1 GEMM + softmax + GEMM sequence
+# Fused wgmma self-attention (csrc/attention.cu) for d_k = 64; ESPB_ATTN=materialized keeps the round-1 GEMM + softmax + GEMM sequence
 # (A/B measurements and the validator of the fused kernel).
 _ATTN_MODE = os.environ.get("ESPB_ATTN", "fused")
 

@@ -111,7 +111,7 @@ class BatchBeamSearch(torch.nn.Module):
     # batches of >= group_min_utts utterances are searched as n_groups independent groups on their own streams (own state, decoder
     # workspace and CUDA graphs), stepped in lock-step from the host so that the groups' kernel chains overlap on the device.
     group_min_utts = 16
-    n_groups = 1      # measured on B200 (64 x 30 s, beam 10): 256 utt/s with 1 group, 247 with 2, 234 with 3, 226 with 4 -- the chains do not overlap profitably
+    n_groups = 1      # one group: the decode-step chains of several groups do not overlap profitably
 
     def _group_bounds(self, U):
         import os

@@ -1,11 +1,11 @@
 """TransformerEncoder (absolute positions, conv2d input layer, pre-LN, ReLU feed-forward) with the reference's constructor /
 state_dict surface -- the encoder of the next scope row (SURVEY.md 8f-1, BASELINE configs[4]).  It composes the kernels of the
-Conformer path (conv1 / implicit-GEMM conv2 / tcgen05 3xTF32 GEMMs / LayerNorm) plus a plain masked softmax.
+Conformer path (conv1 / implicit-GEMM conv2 / wgmma 3xTF32 GEMMs / LayerNorm) plus a plain masked softmax.
 
 Reference: espnet2/asr/encoder/transformer_encoder.py:43-299, legacy/nets/pytorch_backend/transformer/encoder_layer.py:65-126,
 attention.py:77-151,262-265 (default branch), embedding.py:38-95 (PositionalEncoding), subsampling.py:397-474.
 Parity: tests/test_gpu_zz_next.py (reference fixture layer by layer, ragged batch, whole Speech2Text) and tests/test_host_logic_emulated.py; self-attention
-is the fused tcgen05 kernel without the rel-pos term (csrc/attention.cu) at d_k = 64.  Measured: bench.py --workload transformer_24l1024_att_64x30s.
+is the fused wgmma kernel without the rel-pos term (csrc/attention.cu) at d_k = 64.
 """
 import math
 from typing import List, Optional, Tuple
@@ -160,7 +160,7 @@ class TransformerEncoder(torch.nn.Module):
         hbuf = self._buf("h", (2, M, U))
         qkv = self._buf("qkv", (2, M, 3 * D))
         vt = self._buf("vt", (2, B, H, dk, Tp))
-        fused = ops.use_flash_attn(dk)      # one tcgen05 kernel for q k^T + masked softmax + p v (csrc/attention.cu)
+        fused = ops.use_flash_attn(dk)      # one wgmma kernel for q k^T + masked softmax + p v (csrc/attention.cu)
         if not fused:
             sc = self._buf("sc", (B, H, T, Tp))
             probs = self._buf("probs", (2, B, H, T, Tp))

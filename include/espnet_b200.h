@@ -1,4 +1,4 @@
-/* espnet_b200.h -- C ABI of libespnet_b200.so (B200 / sm_100a kernels for ESPnet2's Speech2Text path).
+/* espnet_b200.h -- C ABI of libespnet_b200.so (H100 / sm_90a kernels for ESPnet2's Speech2Text path).
  *
  * The reference has no FFI for this path: its boundary is Python classes + registries + state_dict
  * (SURVEY.md 8b).  Each entry point below replaces the ATen call sequence of one reference function and is
@@ -33,7 +33,7 @@ int espb_device_sm(int* major, int* minor);
  * Replaces torch.matmul / F.linear at: positionwise_feed_forward.py:30-32, attention.py:77-119,146,448-452,
  * convolution.py:66,77 (pointwise convs), subsampling.py:400-406,451 (conv2 as implicit GEMM a_mode=1, embed.out
  * with kob), ctc.py:39 (ctc_lo), transformer_decoder.py:227-234 (output_layer), decoder_layer.py (all Linears).
- * use_tc=1: tcgen05.mma kind::tf32, 3 MMAs per product (A_lo*B_hi + A_hi*B_lo + A_hi*B_hi), TMA operands
+ * use_tc=1: wgmma tf32, 3 MMAs per product (A_lo*B_hi + A_hi*B_lo + A_hi*B_hi), TMA operands
  *           (needs 16-byte aligned bases/strides); use_tc=0: SIMT fp32 FFMA kernel, any strides. */
 typedef struct EspbGemmDesc {
   int M, N, K;
@@ -95,7 +95,7 @@ int espb_relpos_softmax_f32(const float* ac, const float* bd, int B, int H, int 
  * keys j < lens[b], 0 elsewhere; scores [B][H][T][Tp] -> probs hi/lo planes [B][H][T][Tp]. */
 int espb_masked_softmax_f32(const float* scores, int B, int H, int T, int Tp, const int* lens, float sqrt_dk, float* probs, long long probs_plane,
                             cudaStream_t stream);
-/* Fused self-attention for d_k = 64 on tcgen05 (attention.py:416-459 rel-pos, :153-265 plain; scores and probabilities never reach HBM):
+/* Fused self-attention for d_k = 64 on wgmma (attention.py:416-459 rel-pos, :153-265 plain; scores and probabilities never reach HBM):
  * out[b,i,h,:] = softmax_j<len_b( (q[b,i,h,:] . k[b,j,h,:] + bd[b,h,i,T-1-i+j]) / sqrt(d_k) ) . v[b,j,h,:].
  * q / k / out are split (hi/lo plane) tensors (first element at q + q_off / k + k_off) with row strides ldq / ldk / ldo, head h at columns h*64..; vt is the split V^T [B][H][64][Tp]
  * written by espb_v_transpose_f32; bd is the UNSHIFTED (q + pos_bias_v) p^T product [B][H][T][Rp] (rel_shift is applied while loading) or NULL

@@ -1,7 +1,7 @@
 """In-graph latency of the decode-step GEMM shapes (CUDA-graph replay of 100 back-to-back launches, CUDA events).
 
-    python scripts/gemm_microbench.py            # current dispatch
-    ESPB_GEMM_SPLITK=0 python scripts/gemm_microbench.py
+    python scripts/gemm_microbench.py                        # default GEMM mode (tc2)
+    ESPNET_B200_GEMM=tc python scripts/gemm_microbench.py    # without chunked promotion
 """
 import os
 import sys
@@ -13,7 +13,7 @@ from espnet_b200 import ops  # noqa: E402
 
 SHAPES = [(640, 512, 32), (640, 512, 512), (640, 512, 2048), (640, 1536, 512), (640, 2048, 512), (640, 5000, 512), (320, 512, 512), (1280, 512, 512)]
 REPS = 100
-tag = "splitk=" + os.environ.get("ESPB_GEMM_SPLITK", "1")
+tag = "mode=" + ops.gemm_mode()
 for M, N, K in SHAPES:
     a, b = ops.split_from(torch.randn(M, K, device="cuda")), ops.split_from(torch.randn(N, K, device="cuda") / K ** 0.5)
     bias = torch.randn(N, device="cuda")

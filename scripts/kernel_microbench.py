@@ -1,9 +1,6 @@
 """Stand-alone timing of single hot kernels on bench-shaped synthetic data (CUDA events, L2 flushed between launches).
 
     python scripts/kernel_microbench.py softmax|srcattn|selfattn|all [reps]
-
-Also the target for one-kernel ncu captures (scripts/gpu_ncu_micro.sh): a 5000-launch bench step under ncu is expensive,
-one launch of one kernel is not.
 """
 import math
 import os
@@ -118,7 +115,7 @@ if which in ("ffn", "all"):
     bias = torch.randn(N, device=dev)
     out = torch.empty(2, M, N, device=dev)
     alg_bytes = (2 * M * K + 2 * N * K + 2 * M * N) * 4
-    timeit(f"gemm_tf32x3_2cta M{M} N{N} K{K} swish split ({2.0 * M * N * K / 1e12:.3f} TFLOP algorithmic)",
+    timeit(f"gemm_tf32x3 M{M} N{N} K{K} swish split ({2.0 * M * N * K / 1e12:.3f} TFLOP algorithmic)",
            lambda: ops.linear(a, b, out, bias=bias, act=ops.ACT_SWISH, split_out=True), alg_bytes)
 
 if which in ("ac", "all"):

@@ -1,4 +1,4 @@
-"""-m gpu: the fused tcgen05 self-attention kernel (csrc/attention.cu, espb_flash_attn_f32) against an fp64 restatement of
+"""-m gpu: the fused wgmma self-attention kernel (csrc/attention.cu, espb_flash_attn_f32) against an fp64 restatement of
 RelPositionMultiHeadedAttention / MultiHeadedAttention (attention.py:416-459, 391-414, 121-151) on seeded inputs: single and multiple key
 tiles, ragged batches (masked keys, query blocks that are all padding, a 1-frame utterance), T = 937 (the benchmarked length), with and
 without the rel-pos term.  Tolerance: 2e-5 absolute on O(1) context vectors (3xTF32 products, fp32 accumulation)."""
