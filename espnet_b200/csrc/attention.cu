@@ -46,6 +46,27 @@ struct AttnParams {
   float scale;                                   // 1 / sqrt(d_k)
 };
 
+// bd values of one row for the keys key0 + 8j + 0/1, j < 8 (key0 even; row = the row's bd pointer shifted by T-1-i): pairs as one 8-byte
+// load where the row's shift leaves them aligned.  Keys >= len are not read (past the band for the last key tile) and give 0.  Every
+// element of v is written on every call: values kept from the previous tile would stay live across P V and spill.
+__device__ __forceinline__ void load_bd_row(const float* row, int key0, int len, float2 (&v)[8]) {
+  const bool vec = (reinterpret_cast<uintptr_t>(row) & 7) == 0;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int key = key0 + 8 * j;
+    float2 x = make_float2(0.f, 0.f);
+    if (row) {
+      if (vec && key + 1 < len) {
+        x = __ldg(reinterpret_cast<const float2*>(row + key));
+      } else {
+        if (key < len) x.x = __ldg(row + key);
+        if (key + 1 < len) x.y = __ldg(row + key + 1);
+      }
+    }
+    v[j] = x;
+  }
+}
+
 template <bool RELPOS>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 flash_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
@@ -131,6 +152,9 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
   const float scale = p.scale;
   const float* bd_a = nullptr;
   const float* bd_b = nullptr;
+  // rel-pos term of the keys J0 + 8j + 2tq + 0/1 of rows ra / rb: loaded at the top of the key tile, so the latency hides under the wait
+  // for K and S = Q K^T (loading a whole tile ahead would keep 32 more registers live across P V, which then spills)
+  float2 bdv_a[8], bdv_b[8];
   if (RELPOS) {
     const long long head = ((long long)b * p.H + h) * p.T;
     if (ra < p.T) bd_a = p.bd + (head + ra) * p.Rp + (p.T - 1 - ra);
@@ -146,6 +170,10 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
     const int st = t % KV_STAGES;
     const uint32_t ph = (uint32_t)((t / KV_STAGES) & 1);
     const int J0 = t * KB;
+    if (RELPOS) {
+      load_bd_row(bd_a, J0 + 2 * tq, len, bdv_a);
+      load_bd_row(bd_b, J0 + 2 * tq, len, bdv_b);
+    }
     // ---- S = Q K^T
     mbar_wait_spin(k_full + 8 * st, ph);
     const uint32_t kt = k_base + st * KV_STAGE_BYTES;
@@ -177,8 +205,8 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
         const bool ok = key < len;
         float va = s[4 * j + e], vb = s[4 * j + 2 + e];
         if (RELPOS) {
-          if (ok && bd_a) va += __ldg(bd_a + key);
-          if (ok && bd_b) vb += __ldg(bd_b + key);
+          if (ok && bd_a) va += e ? bdv_a[j].y : bdv_a[j].x;
+          if (ok && bd_b) vb += e ? bdv_b[j].y : bdv_b[j].x;
         }
         va = ok ? va : -INFINITY;
         vb = ok ? vb : -INFINITY;

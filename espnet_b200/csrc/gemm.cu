@@ -6,6 +6,7 @@
 //   warps 0-7: two consumer warpgroups; warpgroup g issues the wgmma for rows [64g, 64g+64) of the tile and runs their epilogue
 //              (bias / activation / residual / hi-lo split) straight from the accumulator registers
 //   warp 8   : TMA producer (one elected lane) -> full[s]; the consumers release a stage through empty[s] once its MMAs retired
+// The rel-pos band product (EspbGemmDesc::band_t > 0) has its own persistent kernel, relpos_band_kernel.
 #include <cuda.h>
 #include <limits.h>
 #include <stdio.h>
@@ -43,13 +44,6 @@ __device__ __forceinline__ float epi_value(const EpiArgs& e, float acc, long lon
 }
 
 // ------------------------------------------------------------------ tensor-core kernel
-// rel-pos band (EspbGemmDesc::band_t): a tile of rows [m0, m0+bm) x columns [n0, n0+bn) is needed iff it intersects
-// { (m, n) : T-1-m <= n <= 2T-2-m }.
-__device__ __forceinline__ bool band_skip(int T, int m0, int bm, int n0, int bn) {
-  if (T <= 0) return false;
-  return (n0 + bn - 1 < T - 1 - (m0 + bm - 1)) || (n0 > 2 * T - 2 - m0);
-}
-
 template <int BN>
 __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc, uint32_t accum) {
   if constexpr (BN == 128) wgmma_tf32_ss_n128(d, adesc, bdesc, accum);
@@ -93,10 +87,6 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
   const int bx = blockIdx.z % p.nbx, by = blockIdx.z / p.nbx;
   const int num_kb = (p.K + BK - 1) / BK;
-  if (band_skip(p.band_t, m0, BM, n0, BN)) {   // tile outside the rel-pos band
-    espb::pdl_wait();
-    return;
-  }
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 2); }   // empty: one arrival per consumer warpgroup
@@ -181,6 +171,216 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     const float* r = PROMOTE ? acc : part;
     epi_store2(e, row, col + 8 * j, r[4 * j], r[4 * j + 1], p.M, p.N, vec_ok);
     epi_store2(e, row + 8, col + 8 * j, r[4 * j + 2], r[4 * j + 3], p.M, p.N, vec_ok);
+  }
+}
+
+// ------------------------------------------------------------------ rel-pos band kernel (EspbGemmDesc::band_t > 0)
+// Row m of the band product needs only columns [T-1-m, 2T-2-m] (T = band_t).  A work unit is one (batch slice, 128-row block): its
+// rows of A (hi / lo, all of K <= 128) are loaded once, and the B tiles over the columns the block reaches, [T-1-m_last, 2T-2-m0]
+// (about T + 127 columns), stream through a TMA ring of k-block slots.  The grid is persistent (CTA c takes units c, c + gridDim.x, ...)
+// and each consumer warpgroup keeps two accumulator sets, so the MMAs of column tile n+1 run while the stores of tile n drain.  Only
+// in-band elements are stored.  Per output element the MMA sequence is the generic kernel's (per k8 step a_lo b_hi, a_hi b_lo, a_hi b_hi,
+// one fp32 chain over K <= 128 = one promotion chunk), so the stored values are bit-identical to it.
+constexpr int BAND_MAX_KB = 4;        // K <= 128
+constexpr int BAND_SMEM = 232448;     // dynamic shared memory of the band kernel (the sm_90 maximum)
+constexpr int BAND_THREADS = 384;     // warpgroups 0-1: consumers (two accumulator sets each), warpgroup 2: producer (one warp works)
+
+struct BandTile {
+  int k;        // round-robin ordinal of the work unit within this CTA (unit blockIdx.x + k * gridDim.x); -1: no more work
+  int seq;      // units with tiles this CTA processed before this one: selects the A buffer and its barrier phase (units without
+                // in-band columns are skipped and do not count)
+  int t, nt;    // column tile within the unit, tiles of the unit
+  int m0, n0;   // first row and first column of the tile
+  int bx, by;   // batch slice
+};
+
+// The first unit of this CTA at ordinal >= k that has in-band columns, at its tile 0; seq units with tiles came before it.
+__device__ __forceinline__ void band_unit(const EspbGemmDesc& p, int nmb, int k, int seq, int bn, BandTile& w) {
+  const long long nunits = (long long)nmb * p.nbx * p.nby;
+  for (;; ++k) {
+    const long long u = blockIdx.x + (long long)k * gridDim.x;
+    if (u >= nunits) { w.k = -1; return; }
+    const int mb = (int)(u % nmb), z = (int)(u / nmb);
+    const int m0 = mb * BM, mlast = min(p.M, m0 + BM) - 1;
+    const int lo = max(0, p.band_t - 1 - mlast), hi = min(p.N - 1, 2 * p.band_t - 2 - m0);
+    if (hi < lo) continue;
+    const int n_start = lo & ~7;   // 32-byte aligned columns: the 8 consecutive floats a quad stores fill one sector
+    w.k = k; w.seq = seq; w.t = 0; w.nt = (hi - n_start) / bn + 1; w.m0 = m0; w.n0 = n_start; w.bx = z % p.nbx; w.by = z / p.nbx;
+    return;
+  }
+}
+__device__ __forceinline__ void band_next(const EspbGemmDesc& p, int nmb, int bn, BandTile& w) {
+  if (w.t + 1 < w.nt) { ++w.t; w.n0 += bn; return; }
+  band_unit(p, nmb, w.k + 1, w.seq + 1, bn, w);
+}
+
+__device__ __forceinline__ void st_global_v2_if(float* ptr, float a, float b, bool pred) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %3, 0;\n\t@p st.global.v2.f32 [%0], {%1, %2};\n\t}" ::"l"(ptr), "f"(a), "f"(b), "r"((int)pred)
+               : "memory");
+}
+__device__ __forceinline__ void st_global_if(float* ptr, float a, bool pred) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p st.global.f32 [%0], %1;\n\t}" ::"l"(ptr), "f"(a), "r"((int)pred) : "memory");
+}
+
+// Shared memory: [nabuf A buffers of num_kb x (hi | lo) x 128 rows][stages B slots of (hi | lo) x BN rows][barriers].  With two A
+// buffers the next unit's rows load while the current unit runs; with one, they load once the unit's last MMAs retired.
+// NKB = ceil(K / 32) k-blocks; 128-column tiles keep A and a ring of at least NKB slots in shared memory up to NKB = 3, beyond that the
+// tiles are 64 columns wide.
+template <int NKB>
+constexpr int band_bn() { return NKB <= 3 ? 128 : 64; }
+
+template <int NKB, bool PROMOTE>
+__global__ void __launch_bounds__(BAND_THREADS, 1)
+relpos_band_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, EspbGemmDesc p, int bxm, int bym, int axm,
+                   int aym, int nabuf, int stages) {
+  constexpr int BN = band_bn<NKB>();
+  constexpr int SLOT_BYTES = 2 * BN * 128;   // one k-block of B, hi | lo
+  constexpr int NR = BN / 2;
+  constexpr int num_kb = NKB;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t a_bytes = (uint32_t)num_kb * 2 * A_TILE_BYTES;
+  const uint32_t ring = smem_base + nabuf * a_bytes;
+  const uint32_t full_bar = ring + stages * SLOT_BYTES, empty_bar = full_bar + 8 * stages;
+  const uint32_t a_full = empty_bar + 8 * stages, a_empty = a_full + 16;
+  const int nmb = (p.M + BM - 1) / BM;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < stages; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 2); }
+    for (int i = 0; i < 2; ++i) { mbar_init(a_full + 8 * i, 1); mbar_init(a_empty + 8 * i, 2); }   // empty: one arrival per consumer warpgroup
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
+  }
+  __syncthreads();
+  espb::pdl_trigger();
+  espb::pdl_wait();
+
+  if (warp >= 8) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");   // the producer warpgroup hands its registers to the consumers
+    if (warp == 8 && elect_one_sync()) {
+      int s = 0;
+      uint32_t ph = 0;
+      BandTile w;
+      for (band_unit(p, nmb, 0, 0, BN, w); w.k >= 0; band_next(p, nmb, BN, w)) {
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(empty_bar + 8 * s, ph ^ 1);
+          const uint32_t fb = full_bar + 8 * s, sb = ring + s * SLOT_BYTES;
+          mbar_expect_tx(fb, SLOT_BYTES);
+          tma_load_5d(sb, &tmB, fb, kb * BK, w.n0, w.bx * bxm, w.by * bym, 0);
+          tma_load_5d(sb + BN * 128, &tmB, fb, kb * BK, w.n0, w.bx * bxm, w.by * bym, 1);
+          if (++s == stages) { s = 0; ph ^= 1; }
+        }
+        if (w.t == 0) {   // after the unit's first B tile: with one A buffer this waits until the previous unit's MMAs retired
+          const int ab = w.seq % nabuf;
+          mbar_wait(a_empty + 8 * ab, ((uint32_t)(w.seq / nabuf) & 1) ^ 1);
+          const uint32_t fa = a_full + 8 * ab, sa = smem_base + ab * a_bytes;
+          mbar_expect_tx(fa, a_bytes);
+          for (int kb = 0; kb < num_kb; ++kb) {
+            const int ko = (p.kob > 0) ? kb / p.kob : 0;
+            const int ki = (p.kob > 0) ? kb % p.kob : kb;
+            tma_load_5d(sa + kb * 2 * A_TILE_BYTES, &tmA, fa, ki * BK, w.m0, w.bx * axm + ko, w.by * aym, 0);
+            tma_load_5d(sa + kb * 2 * A_TILE_BYTES + A_TILE_BYTES, &tmA, fa, ki * BK, w.m0, w.bx * axm + ko, w.by * aym, 1);
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int wg = warp >> 2;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  int s = 0, rs = 0;   // ring slot of the next acquire / release
+  uint32_t ph = 0;
+  // MMAs of tile w into d (asynchronous: committed, not waited for)
+  auto issue = [&](const BandTile& w, float (&d)[NR]) {
+    const int ab = w.seq % nabuf;
+    if (w.t == 0) mbar_wait_spin(a_full + 8 * ab, (uint32_t)(w.seq / nabuf) & 1);
+    const uint32_t sa = smem_base + ab * a_bytes + wg * 64 * 128;   // this warpgroup's 64 rows of A
+    // every slot of the tile is waited for before the first MMA: no barrier-wait loop runs while MMAs are in flight
+    uint32_t sb[num_kb];
+#pragma unroll
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait_spin(full_bar + 8 * s, ph);
+      sb[kb] = ring + s * SLOT_BYTES;
+      if (++s == stages) { s = 0; ph ^= 1; }
+    }
+    fence_regs(d);
+    wgmma_fence();
+#pragma unroll
+    for (int kb = 0; kb < num_kb; ++kb) {
+      const uint32_t sak = sa + kb * 2 * A_TILE_BYTES;
+#pragma unroll
+      for (int k = 0; k < BK / 8; ++k) {
+        const uint64_t a_hi = gmma_desc(sak + k * 32), a_lo = gmma_desc(sak + A_TILE_BYTES + k * 32);
+        const uint64_t b_hi = gmma_desc(sb[kb] + k * 32), b_lo = gmma_desc(sb[kb] + BN * 128 + k * 32);
+        wgmma_tf32<BN>(d, a_lo, b_hi, (kb == 0 && k == 0) ? 0u : 1u);   // small terms first
+        wgmma_tf32<BN>(d, a_hi, b_lo, 1u);
+        wgmma_tf32<BN>(d, a_hi, b_hi, 1u);
+      }
+    }
+    wgmma_commit();
+  };
+  // After the MMAs of w retired: hand its B slots (and, after the unit's last tile, its A buffer) back to the producer.
+  auto release = [&](const BandTile& w) {
+    for (int kb = 0; kb < num_kb; ++kb) {
+      if (wg_leader) mbar_arrive_local(empty_bar + 8 * rs);
+      if (++rs == stages) rs = 0;
+    }
+    if (w.t == w.nt - 1 && wg_leader) mbar_arrive_local(a_empty + 8 * (w.seq % nabuf));
+  };
+  // Plain epilogue (alpha * acc) of the in-band elements.  Branch-free (predicated stores): the next tile's MMAs are in flight meanwhile,
+  // and ptxas serialises wgmma whose accumulators stay live across divergent control flow.
+  const bool vec_ok = ((p.ldc & 1) == 0) && ((p.sc_x & 1) == 0) && ((p.sc_y & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 7) == 0);
+  auto store = [&](const BandTile& w, const float (&d)[NR]) {
+    float* const cbase = p.C + (long long)w.by * p.sc_y + (long long)w.bx * p.sc_x;
+    const int row0 = w.m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int col = w.n0 + 2 * (lane & 3);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int row = row0 + 8 * r;
+      float* const crow = cbase + (long long)row * p.ldc;
+      // in-band columns [lo, end); none for rows past M
+      const int lo = p.band_t - 1 - row, end = row < p.M ? min(p.N, 2 * p.band_t - 1 - row) : INT_MIN;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int c = col + 8 * j;
+        float v0 = d[4 * j + 2 * r], v1 = d[4 * j + 2 * r + 1];
+        if (PROMOTE) { v0 = 0.f + v0; v1 = 0.f + v1; }   // the generic kernel's promotion of its single chunk into a zeroed accumulator
+        v0 *= p.alpha; v1 *= p.alpha;
+        const bool in0 = c >= lo && c < end, in1 = c + 1 >= lo && c + 1 < end;
+        const bool pair = vec_ok && in0 && in1;
+        st_global_v2_if(crow + c, v0, v1, pair);
+        st_global_if(crow + c, v0, in0 && !pair);
+        st_global_if(crow + c + 1, v1, in1 && !pair);
+      }
+    }
+  };
+  // Tile cur's MMAs are in flight in dc: retire them, start the next tile's MMAs in dn and store cur while they run.  Returns false after
+  // the last tile.  Between the issue into dn and the wait at the top of the next step the code is straight-line.
+  auto step = [&](BandTile& cur, float (&dc)[NR], float (&dn)[NR]) -> bool {
+    wgmma_wait<0>();
+    fence_regs(dc);
+    BandTile nxt = cur;
+    band_next(p, nmb, BN, nxt);
+    release(cur);
+    if (nxt.k < 0) { store(cur, dc); return false; }
+    issue(nxt, dn);
+    store(cur, dc);
+    cur = nxt;
+    return true;
+  };
+
+  float acc0[NR], acc1[NR];
+  BandTile cur;
+  band_unit(p, nmb, 0, 0, BN, cur);
+  if (cur.k < 0) return;
+  issue(cur, acc0);
+  for (;;) {
+    if (!step(cur, acc0, acc1)) break;
+    if (!step(cur, acc1, acc0)) break;
   }
 }
 
@@ -287,6 +487,33 @@ int num_sms() {
   }
   return n;
 }
+
+template <int NKB, bool PROMOTE>
+int launch_band(const CUtensorMap& tmA, const CUtensorMap& tmB, const EspbGemmDesc& d, int bxm, int bym, int axm, int aym, cudaStream_t stream) {
+  constexpr int BN = band_bn<NKB>();
+  static bool attr_set = false;
+  if (!attr_set) {
+    if (cudaFuncSetAttribute(relpos_band_kernel<NKB, PROMOTE>, cudaFuncAttributeMaxDynamicSharedMemorySize, BAND_SMEM) != cudaSuccess) {
+      espb_set_error("cudaFuncSetAttribute(max dynamic smem) failed (band GEMM)");
+      return ESPB_ERR_CUDA;
+    }
+    attr_set = true;
+  }
+  const int num_kb = NKB;
+  const int a_bytes = num_kb * 2 * A_TILE_BYTES, slot = 2 * BN * 128;
+  const int budget = BAND_SMEM - 1024 - 256;   // alignment slack, barriers
+  const int nabuf = (2 * a_bytes + (num_kb + 1) * slot <= budget) ? 2 : 1;
+  const int stages = min(8, (budget - nabuf * a_bytes) / slot);
+  if (stages < num_kb) { espb_set_error("band GEMM: K too large for the shared-memory ring"); return ESPB_ERR_ARG; }
+  const long long units = (long long)((d.M + BM - 1) / BM) * d.nbx * d.nby;
+  const int grid = (int)(units < num_sms() ? units : num_sms());
+  const int smem = 1024 + nabuf * a_bytes + stages * slot + 16 * stages + 32;
+  if (espb::launch_pdl(relpos_band_kernel<NKB, PROMOTE>, dim3(grid), dim3(BAND_THREADS), smem, stream, tmA, tmB, d, bxm, bym, axm, aym, nabuf,
+                       stages) != cudaSuccess) {
+    espb_set_error(cudaGetErrorString(cudaGetLastError())); return ESPB_ERR_CUDA;
+  }
+  return ESPB_OK;
+}
 }  // namespace
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -362,6 +589,21 @@ int espb_gemm_tc_launch(const EspbGemmDesc& d, cudaStream_t stream, int version)
   }
   if (rc != ESPB_OK) return rc;
   const int bxm = d.sb_x != 0 ? 1 : 0, bym = d.sb_y != 0 ? 1 : 0;
+  // rel-pos band product: the band kernel takes a strided A operand, K <= 128 and the plain epilogue (alpha only); any other band
+  // descriptor runs through the generic kernel below, which computes every element (a superset of the band)
+  if (d.band_t > 0 && d.a_mode == 0 && d.K <= BAND_MAX_KB * BK && !d.bias && !d.R && d.act == espb::ACT_NONE && !d.split_out) {
+    const int nkb = (d.K + BK - 1) / BK;
+    long long dims[5] = {d.K, d.N, bxm ? d.nbx : 1, bym ? d.nby : 1, 2};
+    long long str[4] = {d.ldb, d.sb_x, d.sb_y, d.b_plane};
+    if ((rc = make_map(&tmB, d.B, dims, str, nkb <= 3 ? band_bn<3>() : band_bn<4>())) != ESPB_OK) return rc;
+    const bool pr = version == 2;
+    switch (nkb) {
+      case 1: return pr ? launch_band<1, true>(tmA, tmB, d, bxm, bym, axm, aym, stream) : launch_band<1, false>(tmA, tmB, d, bxm, bym, axm, aym, stream);
+      case 2: return pr ? launch_band<2, true>(tmA, tmB, d, bxm, bym, axm, aym, stream) : launch_band<2, false>(tmA, tmB, d, bxm, bym, axm, aym, stream);
+      case 3: return pr ? launch_band<3, true>(tmA, tmB, d, bxm, bym, axm, aym, stream) : launch_band<3, false>(tmA, tmB, d, bxm, bym, axm, aym, stream);
+      default: return pr ? launch_band<4, true>(tmA, tmB, d, bxm, bym, axm, aym, stream) : launch_band<4, false>(tmA, tmB, d, bxm, bym, axm, aym, stream);
+    }
+  }
   const long long tiles_m = (d.M + BM - 1) / BM, nb = (long long)d.nbx * d.nby;
   // 128-column tiles unless the problem then has fewer tiles than SMs (decode-step shapes): 64-column tiles spread it over more SMs
   const int bn = (d.N <= 64 || tiles_m * ((d.N + 127) / 128) * nb < num_sms()) ? 64 : 128;

@@ -25,7 +25,8 @@ struct EspbGemmDesc {
   float alpha;          // out = R + alpha * act(acc + bias)   (R absent: alpha * act(...))
   int act;              // espb::ACT_*
   int cv_t1h, cv_f1h, cv_cin;  // mode 1: conv1-output half extents and channel count
-  int band_t;           // > 0: only columns n with band_t-1-m <= n <= 2*band_t-2-m are ever read (rel-pos shift): tiles outside are skipped
+  int band_t;           // > 0: rel-pos band product; only elements with band_t-1-m <= n <= 2*band_t-2-m are defined in C afterwards.
+                        //   Tensor-core path: relpos_band_kernel (a_mode 0, K <= 128, epilogue alpha only), else the generic kernel
 };
 
 int espb_gemm_tc_launch(const EspbGemmDesc& d, cudaStream_t stream, int version);  // wgmma (1: plain accumulation, 2: chunked promotion)

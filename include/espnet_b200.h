@@ -49,7 +49,8 @@ typedef struct EspbGemmDesc {
   float alpha;
   int act;
   int cv_t1h, cv_f1h, cv_cin;
-  int band_t;          /* > 0: rel-pos band -- row m only needs columns [band_t-1-m, 2*band_t-2-m]; tiles outside are skipped */
+  int band_t;          /* > 0: rel-pos band -- only elements of row m in columns [band_t-1-m, 2*band_t-2-m] are defined in C afterwards
+                          (the band kernel serves a_mode 0, K <= 128 and the plain epilogue; other descriptors compute all of C) */
 } EspbGemmDesc;
 int espb_gemm_f32(const EspbGemmDesc* d, int use_tc, cudaStream_t stream);
 
