@@ -3,7 +3,7 @@
 Public surface mirrors the reference classes on that path (see SURVEY.md section 8b):
 Speech2Text, ESPnetASRModel, DefaultFrontend, UtteranceMVN, ConformerEncoder, CTC,
 TransformerDecoder, BatchBeamSearch, Hypothesis, TooShortUttError (+ GlobalMVN, the output-side text classes, and the
-TransformerEncoder of the next scope row; CTCPrefixScorer and TransformerDecoder.batch_score implement the reference's scorer protocol,
+TransformerEncoder of the next scope row and the EBranchformerEncoder; CTCPrefixScorer and TransformerDecoder.batch_score implement the reference's scorer protocol,
 ``espnet_b200.integration.register()`` adds the classes to the reference's registries).
 All compute goes through the C-ABI CUDA library ``libespnet_b200.so`` (include/espnet_b200.h).
 """
@@ -11,6 +11,7 @@ from .asr_inference import (ESPnetASRModel, Speech2Text, build_model, build_mode
                             encoder_choices, frontend_choices, normalize_choices)
 from .ctc import CTC, CTCPrefixScorer  # noqa: F401
 from .decoder import TransformerDecoder  # noqa: F401
+from .e_branchformer_encoder import EBranchformerEncoder  # noqa: F401
 from .encoder import ConformerEncoder  # noqa: F401
 from .errors import TooShortUttError  # noqa: F401
 from .frontend import DefaultFrontend, GlobalMVN, LogMel, UtteranceMVN  # noqa: F401

@@ -20,6 +20,7 @@ import yaml
 from . import lib
 from .ctc import CTC
 from .decoder import TransformerDecoder
+from .e_branchformer_encoder import EBranchformerEncoder
 from .encoder import ConformerEncoder
 from .errors import TooShortUttError  # noqa: F401
 from .frontend import DefaultFrontend, GlobalMVN, UtteranceMVN
@@ -34,7 +35,8 @@ frontend_choices = {"default": DefaultFrontend}
 normalize_choices = {"global_mvn": GlobalMVN, "utterance_mvn": UtteranceMVN}
 from .streaming_encoder import ContextualBlockConformerEncoder  # noqa: E402
 
-encoder_choices = {"conformer": ConformerEncoder, "transformer": TransformerEncoder, "contextual_block_conformer": ContextualBlockConformerEncoder}
+encoder_choices = {"conformer": ConformerEncoder, "transformer": TransformerEncoder, "contextual_block_conformer": ContextualBlockConformerEncoder,
+                   "e_branchformer": EBranchformerEncoder}
 decoder_choices = {"transformer": TransformerDecoder}
 
 

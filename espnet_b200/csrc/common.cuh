@@ -18,7 +18,7 @@ void espb_set_error(const char* msg);
 
 namespace espb {
 
-constexpr int ACT_NONE = 0, ACT_RELU = 1, ACT_SWISH = 2;
+constexpr int ACT_NONE = 0, ACT_RELU = 1, ACT_SWISH = 2, ACT_GELU = 3;
 
 // Programmatic dependent launch for the launch-latency-bound decode step (one beam-search step is ~80 small dependent kernels).
 // A kernel launched through launch_pdl may become resident while its stream predecessor still runs; it must execute pdl_wait()
@@ -50,13 +50,18 @@ __device__ __forceinline__ float tf32_lo(float x, float hi) { return __uint_as_f
 __device__ __forceinline__ float apply_act(float v, int act) {
   if (act == ACT_RELU) return fmaxf(v, 0.f);
   if (act == ACT_SWISH) return v / (1.f + __expf(-v));
+  if (act == ACT_GELU) return 0.5f * v * (1.f + erff(v * (float)M_SQRT1_2));
   return v;
 }
 // accurate variants (expf, not __expf) are used where parity with the fp32 reference matters
 __device__ __forceinline__ float swish_acc(float v) { return v / (1.f + expf(-v)); }
+// torch.nn.GELU() default (approximate="none"): the exact erf form.  Not inlined, so that the GEMM epilogues, which inline apply_act_acc at
+// every store, keep the code they had before GELU existed.
+static __device__ __noinline__ float gelu_acc(float v) { return 0.5f * v * (1.f + erff(v * (float)M_SQRT1_2)); }
 __device__ __forceinline__ float apply_act_acc(float v, int act) {
   if (act == ACT_RELU) return fmaxf(v, 0.f);
   if (act == ACT_SWISH) return swish_acc(v);
+  if (act == ACT_GELU) return gelu_acc(v);
   return v;
 }
 

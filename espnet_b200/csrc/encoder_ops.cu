@@ -1,6 +1,6 @@
 // Warp-primitive kernels of the Conformer encoder: LayerNorm, conv1 of the 2-D subsampling, rel-pos
 // attention glue (q+u / q+v, V transpose, rel-shift + masked softmax) and the convolution module's
-// GLU + depthwise conv + BatchNorm(eval) + Swish.  All outputs that feed a GEMM are written as
+// GLU + depthwise conv + BatchNorm(eval) + Swish, and the E-Branchformer's cgMLP gating unit and merge module.  All outputs that feed a GEMM are written as
 // tf32 hi/lo planes (see gemm.h).
 //
 // Reference: espnet2/legacy/nets/pytorch_backend/transformer/{layer_norm,subsampling,attention}.py,
@@ -419,6 +419,110 @@ __global__ void __launch_bounds__(256) glu_dwconv_bn_swish_win_kernel(const floa
   }
 }
 
+// ---------------------------------------------------------------- E-Branchformer: cgMLP gating unit and merge module
+// Per-row LayerNorm statistics of the CSGU gate half h[row][Uh .. 2Uh) (cgmlp.py:68-70, eps 1e-12): one warp per row, the row held in
+// registers (NV values per lane), two-pass mean / variance as layernorm_kernel.  stats[row] = (mean, rstd); rows t >= len_b are skipped
+// (the depthwise conv never reads them).
+template <int NV>
+__global__ void __launch_bounds__(256) csgu_stats_kernel(const float* __restrict__ h, int Tmax, int U, const int* __restrict__ lens, float eps,
+                                                         long long rows, float2* __restrict__ stats) {
+  const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  if ((int)(row % Tmax) >= lens[row / Tmax]) return;
+  const int lane = threadIdx.x & 31, Uh = U >> 1;
+  const float* g = h + row * U + Uh;
+  float v[NV];
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    const int c = lane + i * 32;
+    v[i] = (c < Uh) ? g[c] : 0.f;
+    s += v[i];
+  }
+  const float mean = espb::warp_sum(s) / (float)Uh;
+  float q = 0.f;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    const float d = (lane + i * 32 < Uh) ? v[i] - mean : 0.f;
+    q += d * d;
+  }
+  const float rstd = 1.0f / sqrtf(espb::warp_sum(q) / (float)Uh + eps);
+  if (lane == 0) stats[row] = make_float2(mean, rstd);
+}
+
+// Depthwise Conv1d over time (K taps, zero padding at the utterance's own ends) of a [Tmax][C] channel block that starts at column
+// `coff` of rows with pitch `ld`, in 64-frame x 64-channel tiles; a thread owns one channel and DW_RUN consecutive frames.
+//   GATE (CSGU, cgmlp.py:68-79, identity gate):   out = x_r * (conv(LayerNorm(x_g)) + b), x_r = columns [0, C) of the row; the gate is
+//                                                  normalised while the tile is loaded, so it never reaches global memory.
+//   !GATE (merge, e_branchformer_encoder.py:166-170): out = x + (conv(x) + b) over the concatenated branches.
+// Rows t >= len_b of the split output are 0.  K > 0: taps known at compile time, inputs slide through registers (as
+// glu_dwconv_bn_swish_win_kernel); K == 0: any odd kernel size k_rt, direct loop.  Both run the same fmaf chain over k = 0..K-1.
+template <int K, bool GATE>
+__global__ void __launch_bounds__(256) dwconv_tile_kernel(const float* __restrict__ in, long long ld, int coff, int Tmax, int C,
+                                                          const int* __restrict__ lens, const float2* __restrict__ stats,
+                                                          const float* __restrict__ ln_g, const float* __restrict__ ln_b,
+                                                          const float* __restrict__ w /*[C][K]*/, const float* __restrict__ bias, int k_rt,
+                                                          float* __restrict__ out, long long out_plane) {
+  static_assert(DW_TT == 4 * DW_RUN && DW_CC == 64, "256 threads = 64 channels x 4 runs of DW_RUN frames");
+  extern __shared__ float sm[];  // [(DW_TT + K - 1)][DW_CC] input tile (normalised gate for GATE), zero outside [0, len)
+  const int kk = K > 0 ? K : k_rt;
+  const int b = blockIdx.z, t0 = blockIdx.x * DW_TT, c0 = blockIdx.y * DW_CC;
+  const int len = lens[b], pad = (kk - 1) / 2, rows = DW_TT + kk - 1;
+  for (int i = threadIdx.x; i < rows * DW_CC; i += blockDim.x) {
+    const int r = i / DW_CC, c = c0 + (i % DW_CC), t = t0 - pad + r;
+    float v = 0.f;
+    if (t >= 0 && t < len && c < C) {
+      const long long row = (long long)b * Tmax + t;
+      v = in[row * ld + coff + c];
+      if constexpr (GATE) {
+        const float2 st = stats[row];
+        v = (v - st.x) * st.y * __ldg(ln_g + c) + __ldg(ln_b + c);
+      }
+    }
+    sm[i] = v;
+  }
+  __syncthreads();
+  const int cl = threadIdx.x & 63, run = threadIdx.x >> 6, c = c0 + cl;
+  if (c >= C) return;
+  const float* col = sm + (run * DW_RUN) * DW_CC + cl;
+  const float* wc = w + (long long)c * kk;
+  float acc[DW_RUN];
+#pragma unroll
+  for (int o = 0; o < DW_RUN; ++o) acc[o] = 0.f;
+  if constexpr (K > 0) {
+    float wr[K > 0 ? K : 1];
+#pragma unroll
+    for (int k = 0; k < K; ++k) wr[k] = __ldg(wc + k);
+#pragma unroll
+    for (int r = 0; r < DW_RUN + K - 1; ++r) {
+      const float x = col[r * DW_CC];
+#pragma unroll
+      for (int o = 0; o < DW_RUN; ++o) {
+        if (r - o >= 0 && r - o < K) acc[o] = fmaf(x, wr[r - o], acc[o]);   // resolved at compile time: input r is tap r - o of output o
+      }
+    }
+  } else {
+    for (int k = 0; k < kk; ++k) {
+      const float wk = __ldg(wc + k);
+#pragma unroll
+      for (int o = 0; o < DW_RUN; ++o) acc[o] = fmaf(col[(o + k) * DW_CC], wk, acc[o]);
+    }
+  }
+  const float bc = __ldg(bias + c);
+#pragma unroll
+  for (int o = 0; o < DW_RUN; ++o) {
+    const int t = t0 + run * DW_RUN + o;
+    if (t >= Tmax) break;
+    const long long row = (long long)b * Tmax + t;
+    float z = 0.f;
+    if (t < len) {
+      if constexpr (GATE) z = in[row * ld + c] * (acc[o] + bc);
+      else z = col[(o + pad) * DW_CC] + (acc[o] + bc);
+    }
+    store_split(out + row * C + c, out_plane, z);
+  }
+}
+
 // x[b, t >= len_b, :] = 0 for plain and split buffers (keeps padded rows finite).
 __global__ void zero_pad_rows_kernel(float* __restrict__ x, int Tmax, int D, const int* __restrict__ lens, long long plane, int nplanes) {
   const int b = blockIdx.y;
@@ -632,6 +736,42 @@ int espb_glu_dwconv_bn_swish_f32(const float* y, int B, int Tmax, int C, const i
     const size_t smem = ((size_t)(DW_TT + K - 1) * DW_CC + (size_t)DW_CC * K) * sizeof(float);
     glu_dwconv_bn_swish_kernel<<<grid, 256, smem, stream>>>(y, Tmax, C, lens, dw_w, dw_b, K, bn_a, bn_b, out, out_plane);
   }
+  ESPB_CHECK_LAUNCH();
+  return ESPB_OK;
+}
+
+int espb_csgu_f32(const float* h, int B, int Tmax, int U, const int* lens, const float* ln_g, const float* ln_b, float eps, const float* conv_w,
+                  const float* conv_b, int K, float* stats, float* out, long long out_plane, cudaStream_t stream) {
+  if (K < 1 || (K & 1) == 0 || K > 127) { espb_set_error("csgu: kernel size must be odd and <= 127"); return ESPB_ERR_ARG; }
+  if (U <= 0 || (U & 1) || U / 2 > 2048) { espb_set_error("csgu: U must be even and U/2 in (0, 2048]"); return ESPB_ERR_ARG; }
+  if (B <= 0 || Tmax <= 0) return ESPB_OK;
+  const int Uh = U / 2;
+  const long long rows = (long long)B * Tmax;
+  const unsigned sg = (unsigned)((rows + 7) / 8);
+  float2* st = reinterpret_cast<float2*>(stats);
+  if (Uh <= 256) csgu_stats_kernel<8><<<sg, 256, 0, stream>>>(h, Tmax, U, lens, eps, rows, st);
+  else if (Uh <= 512) csgu_stats_kernel<16><<<sg, 256, 0, stream>>>(h, Tmax, U, lens, eps, rows, st);
+  else if (Uh <= 1024) csgu_stats_kernel<32><<<sg, 256, 0, stream>>>(h, Tmax, U, lens, eps, rows, st);
+  else csgu_stats_kernel<64><<<sg, 256, 0, stream>>>(h, Tmax, U, lens, eps, rows, st);
+  ESPB_CHECK_LAUNCH();
+  const dim3 grid((Tmax + DW_TT - 1) / DW_TT, (Uh + DW_CC - 1) / DW_CC, B);
+  const size_t smem = (size_t)(DW_TT + K - 1) * DW_CC * sizeof(float);
+  if (K == 31) dwconv_tile_kernel<31, true><<<grid, 256, smem, stream>>>(h, U, Uh, Tmax, Uh, lens, st, ln_g, ln_b, conv_w, conv_b, K, out, out_plane);
+  else if (K == 15) dwconv_tile_kernel<15, true><<<grid, 256, smem, stream>>>(h, U, Uh, Tmax, Uh, lens, st, ln_g, ln_b, conv_w, conv_b, K, out, out_plane);
+  else dwconv_tile_kernel<0, true><<<grid, 256, smem, stream>>>(h, U, Uh, Tmax, Uh, lens, st, ln_g, ln_b, conv_w, conv_b, K, out, out_plane);
+  ESPB_CHECK_LAUNCH();
+  return ESPB_OK;
+}
+
+int espb_merge_dwconv_f32(const float* cat, int B, int Tmax, int C2, const int* lens, const float* w, const float* b, int K, float* out,
+                          long long out_plane, cudaStream_t stream) {
+  if (K < 1 || (K & 1) == 0 || K > 127) { espb_set_error("merge dwconv: kernel size must be odd and <= 127"); return ESPB_ERR_ARG; }
+  if (B <= 0 || Tmax <= 0 || C2 <= 0) return ESPB_OK;
+  const dim3 grid((Tmax + DW_TT - 1) / DW_TT, (C2 + DW_CC - 1) / DW_CC, B);
+  const size_t smem = (size_t)(DW_TT + K - 1) * DW_CC * sizeof(float);
+  if (K == 3) dwconv_tile_kernel<3, false><<<grid, 256, smem, stream>>>(cat, C2, 0, Tmax, C2, lens, nullptr, nullptr, nullptr, w, b, K, out, out_plane);
+  else if (K == 31) dwconv_tile_kernel<31, false><<<grid, 256, smem, stream>>>(cat, C2, 0, Tmax, C2, lens, nullptr, nullptr, nullptr, w, b, K, out, out_plane);
+  else dwconv_tile_kernel<0, false><<<grid, 256, smem, stream>>>(cat, C2, 0, Tmax, C2, lens, nullptr, nullptr, nullptr, w, b, K, out, out_plane);
   ESPB_CHECK_LAUNCH();
   return ESPB_OK;
 }

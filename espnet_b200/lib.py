@@ -50,6 +50,8 @@ _SIGS = {
     "espb_flash_attn_f32": [P, L, L, L, P, L, L, L, P, L, I, P, I, P, I, I, I, I, P, L, L, P],
     "espb_glu_dwconv_bn_swish_f32": [P, I, I, I, P, P, P, I, P, P, P, L, P],
     "espb_zero_pad_rows_f32": [P, I, I, I, P, L, I, P],
+    "espb_csgu_f32": [P, I, I, I, P, P, P, F, P, P, I, P, P, L, P],
+    "espb_merge_dwconv_f32": [P, I, I, I, P, P, P, I, P, L, P],
     "espb_cbe_build_chunks_f32": [P, I, I, I, I, I, I, P, I, I, F, P, P, P, P],
     "espb_cbe_ctx_propagate_f32": [P, I, I, I, I, P, P, I, I, P],
     "espb_zero_rows_f32": [P, L, L, L, I, L, I, P],

@@ -10,7 +10,7 @@ import torch
 from . import lib
 from .lib import GemmDesc, call, ptr
 
-ACT_NONE, ACT_RELU, ACT_SWISH = 0, 1, 2
+ACT_NONE, ACT_RELU, ACT_SWISH, ACT_GELU = 0, 1, 2, 3
 
 # GEMM kernel: "tc" = wgmma 3xTF32, "tc2" = wgmma 3xTF32 with chunked fp32 promotion, "simt" = FFMA (bring-up / A-B checks);
 # shapes TMA cannot address always use SIMT.

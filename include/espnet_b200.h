@@ -23,6 +23,7 @@ extern "C" {
 #define ESPB_ACT_NONE 0
 #define ESPB_ACT_RELU 1
 #define ESPB_ACT_SWISH 2
+#define ESPB_ACT_GELU 3
 
 const char* espb_last_error(void);
 int espb_abi_version(void);
@@ -108,6 +109,16 @@ int espb_flash_attn_f32(const float* q, long long q_off, long long q_plane, long
 int espb_glu_dwconv_bn_swish_f32(const float* y, int B, int Tmax, int C, const int* lens, const float* dw_w, const float* dw_b, int K,
                                  const float* bn_a, const float* bn_b, float* out, long long out_plane, cudaStream_t stream);
 int espb_zero_pad_rows_f32(float* x, int B, int Tmax, int D, const int* lens, long long plane, int nplanes, cudaStream_t stream);
+/* E-Branchformer cgMLP gating unit, identity gate (espnet2/asr/layers/cgmlp.py:57-81): h [B][Tmax][U] (channel_proj1 + GELU output, plain)
+ * -> out[b][t][c] = h[..][c] * (dwconv_K(LayerNorm_eps(h[..][U/2 ..]))[t][c] + conv_b[c]) as split [B*Tmax][U/2], U/2 <= 2048.  The conv sees
+ * zeros outside [0, lens[b]); rows t >= lens[b] of out are 0.  stats: caller workspace of 2 * B * Tmax floats (per-row mean / rstd); the
+ * normalised gate itself is never written to memory.  conv_w [U/2][K], K odd <= 127. */
+int espb_csgu_f32(const float* h, int B, int Tmax, int U, const int* lens, const float* ln_g, const float* ln_b, float eps, const float* conv_w,
+                  const float* conv_b, int K, float* stats, float* out, long long out_plane, cudaStream_t stream);
+/* E-Branchformer merge (e_branchformer_encoder.py:166-170): cat [B][Tmax][C2] plain -> out = split(cat + dwconv_K(cat) + b) [B*Tmax][C2],
+ * depthwise over C2 channels with zeros outside [0, lens[b]); rows t >= lens[b] of out are 0.  w [C2][K], K odd <= 127. */
+int espb_merge_dwconv_f32(const float* cat, int B, int Tmax, int C2, const int* lens, const float* w, const float* b, int K, float* out,
+                          long long out_plane, cudaStream_t stream);
 
 /* ---- streaming encoder: contextual block processing (espnet2/asr/encoder/contextual_block_conformer_encoder.py:506-572,
  *      legacy/nets/pytorch_backend/conformer/contextual_block_encoder_layer.py:291-308) ---- */
