@@ -13,26 +13,9 @@ from typing import List
 import torch
 
 from . import ops
+from .layers import LN_EPS, _FFN, _MHA, abs_pos_table
 from .lib import call, ptr
 from .ops import ACT_RELU, _count, layernorm, linear, new_split, split_from
-
-LN_EPS = 1e-12
-
-
-class _MHA(torch.nn.Module):
-    def __init__(self, n_feat):
-        super().__init__()
-        self.linear_q = torch.nn.Linear(n_feat, n_feat)
-        self.linear_k = torch.nn.Linear(n_feat, n_feat)
-        self.linear_v = torch.nn.Linear(n_feat, n_feat)
-        self.linear_out = torch.nn.Linear(n_feat, n_feat)
-
-
-class _FFN(torch.nn.Module):
-    def __init__(self, d, units):
-        super().__init__()
-        self.w_1 = torch.nn.Linear(d, units)
-        self.w_2 = torch.nn.Linear(units, d)
 
 
 class _DecoderLayer(torch.nn.Module):
@@ -43,16 +26,6 @@ class _DecoderLayer(torch.nn.Module):
         self.norm1 = torch.nn.LayerNorm(d, eps=LN_EPS)
         self.norm2 = torch.nn.LayerNorm(d, eps=LN_EPS)
         self.norm3 = torch.nn.LayerNorm(d, eps=LN_EPS)
-
-
-def pos_enc_table(length, d):
-    """PositionalEncoding.extend_pe (embedding.py:62-83)."""
-    pos = torch.arange(0, length, dtype=torch.float32).unsqueeze(1)
-    div = torch.exp(torch.arange(0, d, 2, dtype=torch.float32) * -(math.log(10000.0) / d))
-    pe = torch.zeros(length, d)
-    pe[:, 0::2] = torch.sin(pos * div)
-    pe[:, 1::2] = torch.cos(pos * div)
-    return pe
 
 
 class TransformerDecoder(torch.nn.Module):
@@ -202,7 +175,7 @@ class TransformerDecoder(torch.nn.Module):
     def _pe(self, length):
         key = ("pe", length)
         if key not in self._ws:
-            self._ws[key] = pos_enc_table(length, self.d).to(self.after_norm.weight.device)
+            self._ws[key] = abs_pos_table(length, self.d).to(self.after_norm.weight.device)
         return self._ws[key]
 
     @torch.no_grad()

@@ -1,0 +1,311 @@
+"""Host code the four CUDA-path encoders share: the parameter containers (the reference's attribute names, created in the reference's order so
+that a seeded default init gives the same weights), the sinusoid tables, and ``EncoderBase`` -- the state every encoder has (packed weights,
+workspace, ``after_norm``) and the packing and launches of the blocks they have in common: Conv2dSubsampling, the feed-forward module, the
+convolution module, rel-pos and plain self-attention.  Each encoder module keeps its constructor checks, its layer container, the packing of
+its own weights and its per-layer sequence in ``forward``.
+
+The torch.nn layers are parameter containers only (reference checkpoints load by name); forward never calls them.
+"""
+import math
+
+import torch
+
+from . import ops
+from .errors import TooShortUttError
+from .ops import ACT_RELU, _count, layernorm, linear, split_from
+
+# Launches go through ops.call / ops.ptr / ops.gemm / ops.new_split, looked up at call time: the kernel emulation of the tests
+# (tests/emu_backend.py) replaces them in ops and in each encoder module.
+
+LN_EPS = 1e-12  # transformer/layer_norm.py:22
+
+
+class _MHA(torch.nn.Module):
+    def __init__(self, n_feat):
+        super().__init__()
+        self.linear_q = torch.nn.Linear(n_feat, n_feat)
+        self.linear_k = torch.nn.Linear(n_feat, n_feat)
+        self.linear_v = torch.nn.Linear(n_feat, n_feat)
+        self.linear_out = torch.nn.Linear(n_feat, n_feat)
+
+
+class _PosBias(torch.nn.Module):
+    def __init__(self, n_head, n_feat):
+        super().__init__()
+        d_k = n_feat // n_head
+        self.linear_q = torch.nn.Linear(n_feat, n_feat)
+        self.linear_k = torch.nn.Linear(n_feat, n_feat)
+        self.linear_v = torch.nn.Linear(n_feat, n_feat)
+        self.linear_out = torch.nn.Linear(n_feat, n_feat)
+        self.linear_pos = torch.nn.Linear(n_feat, n_feat, bias=False)
+        self.pos_bias_u = torch.nn.Parameter(torch.Tensor(n_head, d_k))
+        self.pos_bias_v = torch.nn.Parameter(torch.Tensor(n_head, d_k))
+        torch.nn.init.xavier_uniform_(self.pos_bias_u)
+        torch.nn.init.xavier_uniform_(self.pos_bias_v)
+
+
+class _FFN(torch.nn.Module):
+    def __init__(self, d, units):
+        super().__init__()
+        self.w_1 = torch.nn.Linear(d, units)
+        self.w_2 = torch.nn.Linear(units, d)
+
+
+class _ConvModule(torch.nn.Module):
+    def __init__(self, channels, kernel_size):
+        super().__init__()
+        assert (kernel_size - 1) % 2 == 0
+        self.pointwise_conv1 = torch.nn.Conv1d(channels, 2 * channels, 1)
+        self.depthwise_conv = torch.nn.Conv1d(channels, channels, kernel_size, padding=(kernel_size - 1) // 2, groups=channels)
+        self.norm = torch.nn.BatchNorm1d(channels)
+        self.pointwise_conv2 = torch.nn.Conv1d(channels, channels, 1)
+
+
+class _Conv2dSubsampling(torch.nn.Module):
+    """Conv2dSubsampling and Conv2dSubsamplingWOPosEnc: the same parameters (the positional encoding has none)."""
+
+    def __init__(self, idim, odim):
+        super().__init__()
+        self.conv = torch.nn.Sequential(torch.nn.Conv2d(1, odim, 3, 2), torch.nn.ReLU(), torch.nn.Conv2d(odim, odim, 3, 2),
+                                        torch.nn.ReLU())
+        self.out = torch.nn.Linear(odim * (((idim - 1) // 2 - 1) // 2), odim)
+
+
+def _sinusoid_table(pos, d):
+    """Row k = sin / cos of pos[k] * 10000^(-2i/d) in the even / odd columns (embedding.py:62-83)."""
+    pos = pos.unsqueeze(1)
+    div = torch.exp(torch.arange(0, d, 2, dtype=torch.float32) * -(math.log(10000.0) / d))
+    pe = torch.zeros(pos.shape[0], d)
+    pe[:, 0::2] = torch.sin(pos * div)
+    pe[:, 1::2] = torch.cos(pos * div)
+    return pe
+
+
+def abs_pos_table(length, d):
+    """PositionalEncoding.extend_pe (embedding.py:62-83): row t = sinusoid of position t."""
+    return _sinusoid_table(torch.arange(0, length, dtype=torch.float32), d)
+
+
+def rel_pos_table(T, d):
+    """(2T-1, d) slice RelPositionalEncoding.forward returns: row k = sinusoid of relative position T-1-k
+    (embedding.py:286-334).  Built once per length on the host, like the reference's ``pe`` buffer."""
+    return _sinusoid_table(torch.arange(T - 1, -T, -1, dtype=torch.float32), d)
+
+
+def subsampled_len(n):
+    """Lengths after the two 3x3 stride-2 convs of Conv2dSubsampling: (after conv1, after conv2)."""
+    n1 = (n - 3) // 2 + 1
+    return n1, (n1 - 3) // 2 + 1
+
+
+def _pitch(n):
+    """Row pitch of the score / probability matrices: a multiple of 32 floats, so that every 128-byte store segment of the GEMM epilogues
+    is a whole cache line (partial-sector writes cost a DRAM read-modify-write)."""
+    return (n + 31) // 32 * 32
+
+
+class EncoderBase(torch.nn.Module):
+    """``embed`` (Conv2dSubsampling), ``encoders`` (the layers, built from ``layers``) and ``after_norm``, created in this order as in the
+    reference, plus the packed weights and the workspace.  Subclasses set ``heads`` and ``num_blocks`` (and ``kernel`` with the convolution
+    module) and define ``_pack`` and ``forward``."""
+
+    trace = None            # set to a list to collect per-stage outputs (tests)
+    last_split_out = None   # split copy of the last output (feeds the CTC head / decoder memory GEMMs)
+
+    def __init__(self, input_size, output_size, layers):
+        super().__init__()
+        self._output_size, self.idim = output_size, input_size
+        self.embed = _Conv2dSubsampling(input_size, output_size)
+        self.encoders = torch.nn.ModuleList(layers)
+        self.after_norm = torch.nn.LayerNorm(output_size, eps=LN_EPS)
+        self._packed, self._ws = None, {}
+        self._pos_cache = {}   # rel-pos encoders: _pos per length
+
+    def output_size(self) -> int:
+        return self._output_size
+
+    def _load_from_state_dict(self, *args, **kwargs):
+        self._packed = None
+        return super()._load_from_state_dict(*args, **kwargs)
+
+    def _buf(self, name, shape, zero=False, dtype=torch.float32):
+        """Workspace tensor kept across calls; a new shape or dtype replaces the buffer of that name (freed before the allocation)."""
+        key = (name, tuple(shape), dtype)
+        t = self._ws.get(key)
+        if t is None:
+            for k in [k for k in self._ws if k[0] == name]:
+                del self._ws[k]
+            t = (torch.zeros if zero else torch.empty)(shape, dtype=dtype, device=self.after_norm.weight.device)
+            self._ws[key] = t
+        return t
+
+    # ---------------------------------------------------------------- weights -> device-side packed/split form
+    def _f32(self, t):
+        return t.detach().to(device=self.after_norm.weight.device, dtype=torch.float32).contiguous()
+
+    def _pack_ln(self, m):
+        return self._f32(m.weight), self._f32(m.bias)
+
+    def _pack_ffn(self, m):
+        f32 = self._f32
+        return split_from(f32(m.w_1.weight)), f32(m.w_1.bias), split_from(f32(m.w_2.weight)), f32(m.w_2.bias)
+
+    def _pack_mha(self, a):
+        """q / k / v projections fused into one [3D][D] GEMM, linear_out, and the rel-pos biases of a _PosBias."""
+        f32 = self._f32
+        d = dict(qkv_w=split_from(torch.cat([f32(a.linear_q.weight), f32(a.linear_k.weight), f32(a.linear_v.weight)], 0)),
+                 qkv_b=torch.cat([f32(a.linear_q.bias), f32(a.linear_k.bias), f32(a.linear_v.bias)], 0),
+                 out_w=split_from(f32(a.linear_out.weight)), out_b=f32(a.linear_out.bias))
+        if isinstance(a, _PosBias):
+            d["pos_u"], d["pos_v"] = f32(a.pos_bias_u).view(-1), f32(a.pos_bias_v).view(-1)
+        return d
+
+    def _pack_pos(self, attns):
+        """linear_pos of every layer stacked [L*D][D]: one GEMM per length projects the rel-pos table for all layers (_pos)."""
+        return split_from(torch.cat([self._f32(a.linear_pos.weight) for a in attns], 0))
+
+    def _pack_conv(self, cm):
+        f32, D = self._f32, self._output_size
+        d = dict(pw1_w=split_from(f32(cm.pointwise_conv1.weight).view(2 * D, D)), pw1_b=f32(cm.pointwise_conv1.bias),
+                 dw_w=f32(cm.depthwise_conv.weight).view(D, -1), dw_b=f32(cm.depthwise_conv.bias))
+        # BatchNorm1d eval: y = x*alpha + beta with alpha = weight/sqrt(var+eps) (what ATen's CPU kernel computes)
+        inv = 1.0 / torch.sqrt(f32(cm.norm.running_var) + cm.norm.eps)
+        alpha = inv * f32(cm.norm.weight)
+        d["bn_a"], d["bn_b"] = alpha.contiguous(), (f32(cm.norm.bias) - f32(cm.norm.running_mean) * alpha).contiguous()
+        d["pw2_w"], d["pw2_b"] = split_from(f32(cm.pointwise_conv2.weight).view(D, D)), f32(cm.pointwise_conv2.bias)
+        return d
+
+    def _pack_io(self):
+        """Conv2dSubsampling in the layouts of the conv1 kernel and the implicit-GEMM conv2, and after_norm."""
+        f32, e = self._f32, self.embed
+        D = C = self._output_size
+        F1, F2 = subsampled_len(self.idim)
+        return dict(F1=F1, F2=F2, c1_w=f32(e.conv[0].weight).view(C, 9), c1_b=f32(e.conv[0].bias),
+                    # conv2 weight [co][ci][kt][kf] -> [co][(kt*3+kf)*C + ci]
+                    c2_w=split_from(f32(e.conv[2].weight).permute(0, 2, 3, 1).reshape(C, 9 * C)), c2_b=f32(e.conv[2].bias),
+                    # embed.out columns are c*F2+f (subsampling.py:450-451) -> f*C+c to match the [B][F2][T][C] conv2 output
+                    out_w=split_from(f32(e.out.weight).view(D, C, F2).permute(0, 2, 1).reshape(D, F2 * C)), out_b=f32(e.out.bias),
+                    after_norm=self._pack_ln(self.after_norm))
+
+    # ---------------------------------------------------------------- launches
+    def _lengths(self, xs_pad, ilens):
+        """check_short_utt (subsampling.py:43-44) and the subsampled lengths -> (xs_pad fp32 contiguous, T, olens, lens32 on the device).
+
+        The reference decodes one utterance per call, so the limit applies to every utterance of a ragged batch, not to the padded length
+        (an utterance with < 7 frames would get olens 0)."""
+        xs_pad = xs_pad.contiguous().float()
+        B, Tf, F = xs_pad.shape
+        assert F == self.idim
+        min_len = int(torch.as_tensor(ilens).min()) if torch.as_tensor(ilens).numel() else Tf
+        if Tf < 7 or min_len < 7:
+            size = min(Tf, min_len)
+            which = "" if Tf < 7 else f" (utterance {int(torch.as_tensor(ilens).argmin())} of the batch)"
+            raise TooShortUttError(f"has {size} frames and is too short for subsampling (it needs more than 7 frames), "
+                                   f"return empty results{which}", size, 7)
+        olens = torch.div(torch.div(ilens - 1, 2, rounding_mode="trunc") - 1, 2, rounding_mode="trunc")
+        return xs_pad, subsampled_len(Tf)[1], olens, olens.to(device=xs_pad.device, dtype=torch.int32).contiguous()
+
+    def _subsample(self, xs, x, alpha, pe=None):
+        """Conv2dSubsampling (subsampling.py:432-474) of xs (B, T_f, idim) into x [B*T][D]: x = alpha * out(conv(xs)) [+ pe[t]], the
+        positional table entering as a batch-broadcast residual of the embed.out GEMM."""
+        pk = self._packed
+        B, Tf, F = xs.shape
+        D = C = self._output_size
+        F1, F2 = pk["F1"], pk["F2"]
+        T1, T = subsampled_len(Tf)
+        T1h, F1h = (T1 + 1) // 2, (F1 + 1) // 2
+        c1 = self._buf("c1", (B, 8, F1h, T1h, C), zero=True)
+        ops.call("espb_conv1_relu_f32", ops.ptr(xs), B, Tf, F, ops.ptr(pk["c1_w"]), ops.ptr(pk["c1_b"]), C, ops.ptr(c1), T1, F1, T1h, F1h)
+        _count()
+        c2 = self._buf("c2", (2, B, F2, T, C))
+        ops.gemm(T, C, 9 * C, c1, 0, 0, pk["c2_w"], C * 9 * C, 9 * C, c2, C, c_plane=B * F2 * T * C, split_out=True, bias=pk["c2_b"],
+                 act=ACT_RELU, nbx=F2, nby=B, sc=(T * C, F2 * T * C), a_mode=1, conv=(T1h, F1h, C))
+        ops.gemm(T, D, F2 * C, c2, B * F2 * T * C, C, pk["out_w"], D * F2 * C, F2 * C, x, D, bias=pk["out_b"], alpha=alpha, R=pe,
+                 ldr=0 if pe is None else D, nbx=1, nby=B, sa=(T * C, F2 * T * C), sc=(0, T * D), kob=C // 32)
+
+    def _ffn(self, x, xn, norm, weights, act, alpha):
+        """x += alpha * w_2(act(w_1(LN(x))))  (PositionwiseFeedForward behind its pre-LayerNorm)."""
+        w1, b1, w2, b2 = weights
+        h = self._buf("h", (2, x.shape[0], w1.shape[1]))
+        layernorm(x, *norm, LN_EPS, out_split=xn)
+        linear(xn, w1, h, bias=b1, act=act, split_out=True)
+        linear(h, w2, x, bias=b2, residual=x, alpha=alpha)
+
+    def _conv_module(self, x, xn, norm, w, nseq, S, lens):
+        """x += ConvolutionModule(LN(x))  (convolution.py:56-79) over nseq sequences of S rows; sequence b sees zeros outside rows
+        0..lens[b]-1.  GLU, depthwise conv, BatchNorm and swish run as one kernel between the two pointwise GEMMs."""
+        D, M = self._output_size, nseq * S
+        y, cv = self._buf("y", (M, 2 * D)), self._buf("cv", (2, M, D))
+        layernorm(x, *norm, LN_EPS, out_split=xn)
+        linear(xn, w["pw1_w"], y, bias=w["pw1_b"])
+        ops.call("espb_glu_dwconv_bn_swish_f32", ops.ptr(y), nseq, S, D, ops.ptr(lens), ops.ptr(w["dw_w"]), ops.ptr(w["dw_b"]), self.kernel,
+                 ops.ptr(w["bn_a"]), ops.ptr(w["bn_b"]), ops.ptr(cv), M * D)
+        _count()
+        linear(cv, w["pw2_w"], x, bias=w["pw2_b"], residual=x)
+
+    def _pos(self, T):
+        """P_all split [2][2T-1][L*D] = linear_pos(pos_emb) for every layer (one GEMM per length, cached)."""
+        if T not in self._pos_cache:
+            if len(self._pos_cache) > 8:
+                self._pos_cache.clear()
+            D, L = self._output_size, self.num_blocks
+            pe = split_from(rel_pos_table(T, D).to(self.after_norm.weight.device))
+            out = ops.new_split(2 * T - 1, L * D, device=pe.device)
+            linear(pe, self._packed["pos_w_all"], out, split_out=True)
+            self._pos_cache[T] = out
+        return self._pos_cache[T]
+
+    def _relpos_attn(self, qkv, w, li, p_all, ctx, B, T, lens32):
+        """RelPositionMultiHeadedAttention (attention.py:416-459) of layer li, from the fused q|k|v projection qkv (split [2][B*T][3D]) to
+        ctx (split [2][B*T][D]); the output projection is the caller's.  p_all = _pos(T)."""
+        D, H, L = self._output_size, self.heads, self.num_blocks
+        dk, M, R = D // H, B * T, 2 * T - 1
+        Tp, Rp = _pitch(T), _pitch(R)
+        qu, qv = self._buf("qu", (2, M, D)), self._buf("qv", (2, M, D))
+        vt = self._buf("vt", (2, B, H, dk, Tp))
+        bd = self._buf("bd", (B, H, T, Rp))
+        ops.call("espb_qu_qv_f32", ops.ptr(qkv), M * 3 * D, M, D, ops.ptr(w["pos_u"]), ops.ptr(w["pos_v"]), ops.ptr(qu), ops.ptr(qv), M * D)
+        ops.call("espb_v_transpose_f32", ops.ptr(qkv), M * 3 * D, B, T, D, H, ops.ptr(lens32), ops.ptr(vt), B * H * dk * Tp, Tp)
+        _count(2)
+        ops.gemm(T, R, dk, qv, M * D, D, p_all, R * L * D, L * D, bd, Rp, nbx=H, nby=B, sa=(dk, T * D), sb=(dk, 0),
+                 sc=(T * Rp, H * T * Rp), b_off=li * D, band_t=T)   # rel_shift only ever reads bd[i][T-1-i .. 2T-2-i]
+        if ops.use_flash_attn(dk):      # one wgmma kernel for q k^T + rel_shift + softmax + p v (csrc/attention.cu); else materialised
+            ops.flash_attn(qu, 0, D, qkv, D, 3 * D, vt, Tp, bd, Rp, lens32, B, H, T, dk, ctx)
+        else:
+            ac, probs = self._buf("ac", (B, H, T, Tp)), self._buf("probs", (2, B, H, T, Tp))
+            ops.gemm(T, T, dk, qu, M * D, D, qkv, M * 3 * D, 3 * D, ac, Tp, nbx=H, nby=B, sa=(dk, T * D), sb=(dk, T * 3 * D),
+                     sc=(T * Tp, H * T * Tp), b_off=D)
+            ops.call("espb_relpos_softmax_f32", ops.ptr(ac), ops.ptr(bd), B, H, T, Tp, Rp, ops.ptr(lens32), math.sqrt(dk), ops.ptr(probs),
+                     B * H * T * Tp)
+            _count()
+            ops.gemm(T, dk, T, probs, B * H * T * Tp, Tp, vt, B * H * dk * Tp, Tp, ctx, D, c_plane=M * D, split_out=True, nbx=H, nby=B,
+                     sa=(T * Tp, H * T * Tp), sb=(dk * Tp, H * dk * Tp), sc=(dk, T * D))
+
+    def _attn(self, qkv, ctx, nseq, S, lens, fused):
+        """MultiHeadedAttention (attention.py:77-151) over nseq sequences of S rows, from the fused q|k|v projection qkv (split
+        [2][nseq*S][3D]) to ctx (split [2][nseq*S][D]); sequence b attends its keys 0..lens[b]-1.  fused: one wgmma kernel for q k^T + masked
+        softmax + p v (csrc/attention.cu); else scores and probabilities are materialised.  The output projection is the caller's."""
+        D, H = self._output_size, self.heads
+        dk, M, Sp = D // H, nseq * S, _pitch(S)
+        vt = self._buf("vt", (2, nseq, H, dk, Sp))
+        ops.call("espb_v_transpose_f32", ops.ptr(qkv), M * 3 * D, nseq, S, D, H, ops.ptr(lens), ops.ptr(vt), nseq * H * dk * Sp, Sp)
+        _count()
+        if fused:
+            ops.flash_attn(qkv, 0, 3 * D, qkv, D, 3 * D, vt, Sp, None, 0, lens, nseq, H, S, dk, ctx)
+        else:
+            sc, probs = self._buf("sc", (nseq, H, S, Sp)), self._buf("probs", (2, nseq, H, S, Sp))
+            ops.gemm(S, S, dk, qkv, M * 3 * D, 3 * D, qkv, M * 3 * D, 3 * D, sc, Sp, nbx=H, nby=nseq, sa=(dk, S * 3 * D), sb=(dk, S * 3 * D),
+                     sc=(S * Sp, H * S * Sp), b_off=D)
+            ops.call("espb_masked_softmax_f32", ops.ptr(sc), nseq, H, S, Sp, ops.ptr(lens), math.sqrt(dk), ops.ptr(probs), nseq * H * S * Sp)
+            _count()
+            ops.gemm(S, dk, S, probs, nseq * H * S * Sp, Sp, vt, nseq * H * dk * Sp, Sp, ctx, D, c_plane=M * D, split_out=True, nbx=H, nby=nseq,
+                     sa=(S * Sp, H * S * Sp), sb=(dk * Sp, H * dk * Sp), sc=(dk, S * D))
+
+    def _output(self, x, B, T):
+        """after_norm into a new (B, T, D) tensor and its split copy (last_split_out) -> (out, out_split)."""
+        D = self._output_size
+        out = torch.empty(B, T, D, dtype=torch.float32, device=x.device)
+        out_split = self._buf("enc_split", (2, B * T, D))
+        layernorm(x, *self._packed["after_norm"], LN_EPS, out_plain=out, out_split=out_split)
+        self.last_split_out = (out.data_ptr(), out_split)
+        return out, out_split

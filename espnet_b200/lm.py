@@ -17,7 +17,7 @@ from typing import Any, List, Tuple
 
 import torch
 
-from .decoder import _FFN, _MHA, LN_EPS, pos_enc_table
+from .layers import LN_EPS, _FFN, _MHA, abs_pos_table
 from .lib import call, ptr
 from .ops import ACT_RELU, _count, layernorm, linear, new_split, split_from
 
@@ -103,7 +103,7 @@ class TransformerLM(torch.nn.Module):
         if self.pos_enc == "sinusoidal":
             key = ("pe", max_len)
             if key not in self._ws:
-                self._ws[key] = pos_enc_table(max_len, D).to(self.decoder.weight.device)
+                self._ws[key] = abs_pos_table(max_len, D).to(self.decoder.weight.device)
             pe = self._ws[key]
         return dict(n=n_slots, max_len=max_len, kc=self._buf("kc", (L, max_len, n_slots, D)), vc=self._buf("vc", (L, max_len, n_slots, D)), pe=pe)
 

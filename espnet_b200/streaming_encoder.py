@@ -10,25 +10,19 @@ and the same ``forward(xs_pad, ilens, prev_states, is_final, infer_mode=True) ->
 What differs: the reference asserts batch size 1 (one Python object per stream); here the batch dimension is a set of N live streams that push
 equally long chunks in lock step, and all of their blocks run through the kernels together (N * blocks sequences of block_size + 2 tokens).
 Only ``forward_infer`` exists (inference); supported configuration: input_layer "conv2d", normalize_before, cnn module, init_average, abs-pos
-self-attention (what ``ContextualBlockConformerEncoder`` builds), macaron optional.
+self-attention (what ``ContextualBlockConformerEncoder`` builds), macaron optional.  The subsampling (Conv2dSubsamplingWOPosEnc has the
+parameters of Conv2dSubsampling), FFN, convolution module and masked self-attention are the shared ones of layers.py.
 """
 import math
 from typing import Optional, Tuple
 
 import torch
 
-from . import ops
-from .decoder import pos_enc_table
-from .encoder import LN_EPS, _ConvModule, _FFN
+from .layers import LN_EPS, EncoderBase, _ConvModule, _FFN, _MHA, abs_pos_table, subsampled_len
+# gemm stays importable here although the shared code in layers.py launches the GEMMs: the kernel emulation of the tests replaces
+# it in every encoder module
 from .lib import call, ptr
-from .ops import ACT_RELU, ACT_SWISH, _count, gemm, layernorm, linear, split_from
-
-
-class _MHA(torch.nn.Module):
-    def __init__(self, d):
-        super().__init__()
-        self.linear_q, self.linear_k = torch.nn.Linear(d, d), torch.nn.Linear(d, d)
-        self.linear_v, self.linear_out = torch.nn.Linear(d, d), torch.nn.Linear(d, d)
+from .ops import ACT_RELU, _count, gemm, layernorm, linear  # noqa: F401
 
 
 class _CBLayer(torch.nn.Module):
@@ -46,14 +40,7 @@ class _CBLayer(torch.nn.Module):
         self.norm_final = torch.nn.LayerNorm(d, eps=LN_EPS)
 
 
-class _Conv2dSubsamplingWOPosEnc(torch.nn.Module):
-    def __init__(self, idim, odim):
-        super().__init__()
-        self.conv = torch.nn.Sequential(torch.nn.Conv2d(1, odim, 3, 2), torch.nn.ReLU(), torch.nn.Conv2d(odim, odim, 3, 2), torch.nn.ReLU())
-        self.out = torch.nn.Linear(odim * (((idim - 1) // 2 - 1) // 2), odim)
-
-
-class ContextualBlockConformerEncoder(torch.nn.Module):
+class ContextualBlockConformerEncoder(EncoderBase):
     def __init__(self, input_size: int, output_size: int = 256, attention_heads: int = 4, linear_units: int = 2048, num_blocks: int = 6,
                  dropout_rate: float = 0.1, positional_dropout_rate: float = 0.1, attention_dropout_rate: float = 0.0,
                  input_layer: Optional[str] = "conv2d", normalize_before: bool = True, concat_after: bool = False,
@@ -61,7 +48,6 @@ class ContextualBlockConformerEncoder(torch.nn.Module):
                  pos_enc_class=None, selfattention_layer_type: str = "rel_selfattn", activation_type: str = "swish", use_cnn_module: bool = True,
                  cnn_module_kernel: int = 31, padding_idx: int = -1, block_size: int = 40, hop_size: int = 16, look_ahead: int = 16,
                  init_average: bool = True, ctx_pos_enc: bool = True):
-        super().__init__()
         bad = []
         if input_layer != "conv2d": bad.append(f"input_layer={input_layer}")
         if not normalize_before or concat_after or not use_cnn_module: bad.append("non pre-LN / concat_after / no cnn module")
@@ -71,133 +57,54 @@ class ContextualBlockConformerEncoder(torch.nn.Module):
         if bad:
             raise NotImplementedError("espnet_b200 ContextualBlockConformerEncoder: " + ", ".join(bad))
         assert output_size % attention_heads == 0 and output_size % 32 == 0
-        self._output_size, self.heads, self.units, self.num_blocks = output_size, attention_heads, linear_units, num_blocks
-        self.kernel, self.idim, self.macaron = cnn_module_kernel, input_size, macaron_style
+        super().__init__(input_size, output_size,
+                         (_CBLayer(output_size, linear_units, cnn_module_kernel, macaron_style) for _ in range(num_blocks)))
+        self.heads, self.num_blocks, self.kernel, self.macaron = attention_heads, num_blocks, cnn_module_kernel, macaron_style
         self.block_size, self.hop_size, self.look_ahead, self.subsample = block_size, hop_size, look_ahead, 4
-        self.embed = _Conv2dSubsamplingWOPosEnc(input_size, output_size)
-        self.encoders = torch.nn.ModuleList(_CBLayer(output_size, linear_units, cnn_module_kernel, macaron_style) for _ in range(num_blocks))
-        self.after_norm = torch.nn.LayerNorm(output_size, eps=LN_EPS)
-        self._packed, self._ws, self._pe = None, {}, None
-
-    def output_size(self) -> int:
-        return self._output_size
-
-    def _load_from_state_dict(self, *args, **kwargs):
-        self._packed = None
-        return super()._load_from_state_dict(*args, **kwargs)
+        self._pe = None
 
     def _pack(self):
-        dev = self.after_norm.weight.device
-        D = C = self._output_size
-        f32 = lambda t: t.detach().to(device=dev, dtype=torch.float32).contiguous()  # noqa: E731
-        e = self.embed
-        F1 = (self.idim - 3) // 2 + 1
-        F2 = (F1 - 3) // 2 + 1
-        pk = dict(F1=F1, F2=F2, c1_w=f32(e.conv[0].weight).view(C, 9), c1_b=f32(e.conv[0].bias),
-                  c2_w=split_from(f32(e.conv[2].weight).permute(0, 2, 3, 1).reshape(C, 9 * C)), c2_b=f32(e.conv[2].bias),
-                  out_w=split_from(f32(e.out.weight).view(D, C, F2).permute(0, 2, 1).reshape(D, F2 * C)), out_b=f32(e.out.bias), layers=[])
+        pk = self._pack_io()
+        layers = []
         for lyr in self.encoders:
-            a, cm = lyr.self_attn, lyr.conv_module
-            d = {nm: (f32(getattr(lyr, nm).weight), f32(getattr(lyr, nm).bias)) for nm in ("norm1", "norm2", "norm_conv", "norm_final")}
-            for nm in ("feed_forward_macaron", "feed_forward"):
-                m = getattr(lyr, nm)
-                d[nm] = None if m is None else (split_from(f32(m.w_1.weight)), f32(m.w_1.bias), split_from(f32(m.w_2.weight)), f32(m.w_2.bias))
-            if lyr.feed_forward_macaron is not None:
-                d["norm_ff_macaron"] = (f32(lyr.norm_ff_macaron.weight), f32(lyr.norm_ff_macaron.bias))
-            d["qkv_w"] = split_from(torch.cat([f32(a.linear_q.weight), f32(a.linear_k.weight), f32(a.linear_v.weight)], 0))
-            d["qkv_b"] = torch.cat([f32(a.linear_q.bias), f32(a.linear_k.bias), f32(a.linear_v.bias)], 0)
-            d["out_w"], d["out_b"] = split_from(f32(a.linear_out.weight)), f32(a.linear_out.bias)
-            d["pw1_w"], d["pw1_b"] = split_from(f32(cm.pointwise_conv1.weight).view(2 * D, D)), f32(cm.pointwise_conv1.bias)
-            d["dw_w"], d["dw_b"] = f32(cm.depthwise_conv.weight).view(D, -1), f32(cm.depthwise_conv.bias)
-            inv = 1.0 / torch.sqrt(f32(cm.norm.running_var) + cm.norm.eps)
-            alpha = inv * f32(cm.norm.weight)
-            d["bn_a"], d["bn_b"] = alpha.contiguous(), (f32(cm.norm.bias) - f32(cm.norm.running_mean) * alpha).contiguous()
-            d["pw2_w"], d["pw2_b"] = split_from(f32(cm.pointwise_conv2.weight).view(D, D)), f32(cm.pointwise_conv2.bias)
-            pk["layers"].append(d)
-        pk["after_norm"] = (f32(self.after_norm.weight), f32(self.after_norm.bias))
+            d = {nm: self._pack_ln(getattr(lyr, nm)) for nm in ("norm1", "norm2", "norm_conv", "norm_final")}
+            if self.macaron:
+                d["norm_ff_macaron"], d["feed_forward_macaron"] = self._pack_ln(lyr.norm_ff_macaron), self._pack_ffn(lyr.feed_forward_macaron)
+            d["feed_forward"] = self._pack_ffn(lyr.feed_forward)
+            d.update(self._pack_mha(lyr.self_attn), **self._pack_conv(lyr.conv_module))
+            layers.append(d)
+        pk["layers"] = layers
         self._packed = pk
         return pk
 
-    def _buf(self, name, shape, zero=False, dtype=torch.float32):
-        key = (name, tuple(shape), dtype)
-        t = self._ws.get(key)
-        if t is None:
-            for k in [k for k in self._ws if k[0] == name]:
-                del self._ws[k]
-            t = (torch.zeros if zero else torch.empty)(shape, dtype=dtype, device=self.after_norm.weight.device)
-            self._ws[key] = t
-        return t
-
     def _pe_table(self, need):
         if self._pe is None or self._pe.shape[0] < need:
-            self._pe = pos_enc_table(max(5000, 2 * need), self._output_size).to(self.after_norm.weight.device)
+            self._pe = abs_pos_table(max(5000, 2 * need), self._output_size).to(self.after_norm.weight.device)
         return self._pe
-
-    # ---------------------------------------------------------------- subsampling: Conv2dSubsamplingWOPosEnc (no scaling, no pos-enc)
-    def _embed(self, xs, pk):
-        N, Tf, F = xs.shape
-        D = C = self._output_size
-        F1, F2 = pk["F1"], pk["F2"]
-        T1 = (Tf - 3) // 2 + 1
-        T = (T1 - 3) // 2 + 1
-        T1h, F1h = (T1 + 1) // 2, (F1 + 1) // 2
-        c1 = self._buf("c1", (N, 8, F1h, T1h, C), zero=True)
-        call("espb_conv1_relu_f32", ptr(xs), N, Tf, F, ptr(pk["c1_w"]), ptr(pk["c1_b"]), C, ptr(c1), T1, F1, T1h, F1h)
-        _count()
-        c2 = self._buf("c2", (2, N, F2, T, C))
-        gemm(T, C, 9 * C, c1, 0, 0, pk["c2_w"], C * 9 * C, 9 * C, c2, C, c_plane=N * F2 * T * C, split_out=True, bias=pk["c2_b"], act=ACT_RELU,
-             nbx=F2, nby=N, sc=(T * C, F2 * T * C), a_mode=1, conv=(T1h, F1h, C))
-        x = torch.empty(N, T, D, dtype=torch.float32, device=xs.device)
-        gemm(T, D, F2 * C, c2, N * F2 * T * C, C, pk["out_w"], D * F2 * C, F2 * C, x, D, bias=pk["out_b"], nbx=1, nby=N,
-             sa=(T * C, F2 * T * C), sc=(0, T * D), kob=C // 32)
-        return x
 
     # ---------------------------------------------------------------- the layers over nseq sequences of S tokens
     def _layers(self, x, nseq, S, pk, n_keys, zero_query0, past_ctx, N, nb):
         """x [nseq*S][D] in place.  n_keys: keys 0..n_keys-1 of every sequence are attended (the block mask lets tokens 1..S-1 see tokens
         0..S-2, contextual_block_conformer_encoder.py:543-549); zero_query0: token 0 attends nothing.  Returns next_ctx [N][L][D] or None."""
-        D, H, U, K, L = self._output_size, self.heads, self.units, self.kernel, self.num_blocks
-        dk, M = D // H, nseq * S
-        dev = x.device
-        Sp = (S + 31) // 32 * 32
+        D, L, M = self._output_size, self.num_blocks, nseq * S
         lens_k = self._buf("lens_k", (nseq,), dtype=torch.int32); lens_k.fill_(n_keys)
         lens_all = self._buf("lens_all", (nseq,), dtype=torch.int32); lens_all.fill_(S)
-        xn, hbuf = self._buf("xn", (2, M, D)), self._buf("h", (2, M, U))
-        qkv, vt = self._buf("qkv", (2, M, 3 * D)), self._buf("vt", (2, nseq, H, dk, Sp))
-        sc, probs = self._buf("sc", (nseq, H, S, Sp)), self._buf("probs", (2, nseq, H, S, Sp))
-        ctx, y, cv = self._buf("ctx", (2, M, D)), self._buf("y", (M, 2 * D)), self._buf("cv", (2, M, D))
-        next_ctx = torch.zeros(N, L, D, dtype=torch.float32, device=dev) if zero_query0 else None
+        xn, qkv, ctx = self._buf("xn", (2, M, D)), self._buf("qkv", (2, M, 3 * D)), self._buf("ctx", (2, M, D))
+        next_ctx = torch.zeros(N, L, D, dtype=torch.float32, device=x.device) if zero_query0 else None
         ff_scale = 0.5 if self.macaron else 1.0
+        # PositionwiseFeedForward's default ReLU: the encoder passes no activation (:163-168)
         for li, w in enumerate(pk["layers"]):
             if self.macaron:
-                w1, b1, w2, b2 = w["feed_forward_macaron"]
-                layernorm(x, *w["norm_ff_macaron"], LN_EPS, out_split=xn)
-                linear(xn, w1, hbuf, bias=b1, act=ACT_RELU, split_out=True)   # PositionwiseFeedForward's default ReLU (the encoder passes no activation, :163-168)
-                linear(hbuf, w2, x, bias=b2, residual=x, alpha=ff_scale)
+                self._ffn(x, xn, w["norm_ff_macaron"], w["feed_forward_macaron"], ACT_RELU, ff_scale)
             layernorm(x, *w["norm1"], LN_EPS, out_split=xn)
             linear(xn, w["qkv_w"], qkv, bias=w["qkv_b"], split_out=True)
-            call("espb_v_transpose_f32", ptr(qkv), M * 3 * D, nseq, S, D, H, ptr(lens_k), ptr(vt), nseq * H * dk * Sp, Sp)
-            _count()
-            gemm(S, S, dk, qkv, M * 3 * D, 3 * D, qkv, M * 3 * D, 3 * D, sc, Sp, nbx=H, nby=nseq, sa=(dk, S * 3 * D), sb=(dk, S * 3 * D),
-                 sc=(S * Sp, H * S * Sp), b_off=D)
-            call("espb_masked_softmax_f32", ptr(sc), nseq, H, S, Sp, ptr(lens_k), math.sqrt(dk), ptr(probs), nseq * H * S * Sp)
-            _count()
-            gemm(S, dk, S, probs, nseq * H * S * Sp, Sp, vt, nseq * H * dk * Sp, Sp, ctx, D, c_plane=M * D, split_out=True, nbx=H, nby=nseq,
-                 sa=(S * Sp, H * S * Sp), sb=(dk * Sp, H * dk * Sp), sc=(dk, S * D))
+            self._attn(qkv, ctx, nseq, S, lens_k, False)
             if zero_query0:   # the block mask has no key for token 0: its attention output is zero (masked_fill after the softmax)
                 call("espb_zero_rows_f32", ptr(ctx), 0, S, nseq, D, M * D, 2)
                 _count()
             linear(ctx, w["out_w"], x, bias=w["out_b"], residual=x)
-            layernorm(x, *w["norm_conv"], LN_EPS, out_split=xn)
-            linear(xn, w["pw1_w"], y, bias=w["pw1_b"])
-            call("espb_glu_dwconv_bn_swish_f32", ptr(y), nseq, S, D, ptr(lens_all), ptr(w["dw_w"]), ptr(w["dw_b"]), K, ptr(w["bn_a"]),
-                 ptr(w["bn_b"]), ptr(cv), M * D)
-            _count()
-            linear(cv, w["pw2_w"], x, bias=w["pw2_b"], residual=x)
-            w1, b1, w2, b2 = w["feed_forward"]
-            layernorm(x, *w["norm2"], LN_EPS, out_split=xn)
-            linear(xn, w1, hbuf, bias=b1, act=ACT_RELU, split_out=True)   # PositionwiseFeedForward's default ReLU (the encoder passes no activation, :163-168)
-            linear(hbuf, w2, x, bias=b2, residual=x, alpha=ff_scale)
+            self._conv_module(x, xn, w["norm_conv"], w, nseq, S, lens_all)
+            self._ffn(x, xn, w["norm2"], w["feed_forward"], ACT_RELU, ff_scale)
             layernorm(x, *w["norm_final"], LN_EPS, out_plain=x)
             if zero_query0:
                 call("espb_cbe_ctx_propagate_f32", ptr(x), N, nb, S, D, ptr(past_ctx), ptr(next_ctx), li, L)
@@ -242,7 +149,11 @@ class ContextualBlockConformerEncoder(torch.nn.Module):
             n_res = xs_pad.shape[1] % self.subsample + self.subsample * 2
             buf_before = xs_pad[:, xs_pad.shape[1] - n_res:].contiguous()
             xs_pad = xs_pad[:, : n_samples * self.subsample].contiguous()
-        xs = self._embed(xs_pad, pk) if xs_pad.shape[1] >= 7 else xs_pad.new_zeros(N, 0, D)
+        if xs_pad.shape[1] >= 7:   # Conv2dSubsamplingWOPosEnc: no scaling, no positional encoding
+            xs = torch.empty(N, subsampled_len(xs_pad.shape[1])[1], D, dtype=torch.float32, device=dev)
+            self._subsample(xs_pad, xs, 1.0)
+        else:
+            xs = xs_pad.new_zeros(N, 0, D)
         if buf_after is not None:
             xs = torch.cat([buf_after, xs], dim=1)
         total = xs.shape[1]
