@@ -15,7 +15,7 @@ from .e_branchformer_encoder import EBranchformerEncoder  # noqa: F401
 from .encoder import ConformerEncoder  # noqa: F401
 from .errors import TooShortUttError  # noqa: F401
 from .frontend import DefaultFrontend, GlobalMVN, LogMel, UtteranceMVN  # noqa: F401
-from .lm import TransformerLM, build_lm_from_file  # noqa: F401
+from .lm import SequentialRNNLM, TransformerLM, build_lm_from_file  # noqa: F401
 from .search import BatchBeamSearch, Hypothesis  # noqa: F401
 from .search_online import BatchBeamSearchOnline, LengthBonus  # noqa: F401
 from .asr_inference_streaming import Speech2TextStreaming  # noqa: F401

@@ -1115,6 +1115,59 @@ __global__ void track_scores_kernel(const int* __restrict__ parent, const int* _
   if (logp_b) { new_b[ns] = vb; hist_b[(long long)step * n + ns] = vb; }
 }
 
+// ---------------------------------------------------------------- LSTM LM (espnet2/lm/seq_rnn_lm.py: Embedding -> nn.LSTM -> Linear)
+// Recurrent state ring h, c [2][L][n][Hp]: step pos reads its parent from ring (pos-1)&1 at slot anc[s][pos-1] and writes ring pos&1 at
+// slot s (zeros at pos 0).  Layer l's GEMM operand is the split [2][n][Kp_l] = [input | parent h]: Kp_0 = Ep + Hp, Kp_l = 2 Hp; the
+// operands lie back to back in one buffer.  Pad columns are never written here (the host zeroes them once).
+__device__ __forceinline__ int rnnlm_parent(const int* anc, int anc_ld, int pos, int s) {
+  return pos > 0 ? anc[(long long)s * anc_ld + pos - 1] : -1;
+}
+
+// Embedding row of the newest token -> layer 0's input half; every layer's parent h -> that layer's recurrent half.
+__global__ void rnnlm_gather_kernel(const int* __restrict__ tok, const float* __restrict__ emb, int E, int Ep, const int* __restrict__ anc,
+                                    int anc_ld, int pos, const int* __restrict__ step_ptr, const float* __restrict__ h_ring, int L, int n, int H,
+                                    int Hp, float* __restrict__ xs) {
+  espb::pdl_trigger();
+  espb::pdl_wait();
+  if (step_ptr) pos += *step_ptr;
+  const int s = blockIdx.x;
+  const long long kp0 = Ep + Hp, kp1 = 2LL * Hp;
+  const float* e = emb + (long long)tok[s] * E;
+  for (int c = threadIdx.x; c < E; c += blockDim.x) store_split(xs + s * kp0 + c, n * kp0, e[c]);
+  const int p = rnnlm_parent(anc, anc_ld, pos, s);
+  const float* hp = h_ring + (long long)((pos - 1) & 1) * L * n * Hp;
+  for (int l = 0; l < L; ++l) {
+    const long long kp = l ? kp1 : kp0;
+    float* x = xs + (l ? 2LL * n * kp0 + 2LL * (l - 1) * n * kp1 : 0LL) + s * kp + (l ? Hp : Ep);
+    const float* src = hp + ((long long)l * n + (p < 0 ? 0 : p)) * Hp;
+    for (int c = threadIdx.x; c < H; c += blockDim.x) store_split(x + c, n * kp, p < 0 ? 0.f : src[c]);
+  }
+}
+
+__device__ __forceinline__ float sigmoid_acc(float v) { return 1.f / (1.f + expf(-v)); }
+
+// gates [n][4H] (i, f, g, o, biases included) + parent c -> c' = σ(f) c + σ(i) tanh(g), h' = σ(o) tanh(c') into ring pos&1 (plain), and h'
+// split into the next consumer's operand out[s * out_ld + j].
+__global__ void lstm_cell_kernel(const float* __restrict__ gates, const int* __restrict__ anc, int anc_ld, int pos, const int* __restrict__ step_ptr,
+                                 float* __restrict__ h_ring, float* __restrict__ c_ring, int layer, int L, int n, int H, int Hp,
+                                 float* __restrict__ out, long long out_plane, int out_ld) {
+  espb::pdl_trigger();
+  espb::pdl_wait();
+  if (step_ptr) pos += *step_ptr;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)n * H) return;
+  const int s = (int)(i / H), j = (int)(i % H);
+  const float* g = gates + (long long)s * 4 * H + j;
+  const int p = rnnlm_parent(anc, anc_ld, pos, s);
+  const float cp = p < 0 ? 0.f : c_ring[((long long)((pos - 1) & 1) * L + layer) * n * Hp + (long long)p * Hp + j];
+  const float c = sigmoid_acc(g[H]) * cp + sigmoid_acc(g[0]) * tanhf(g[2 * H]);
+  const float h = sigmoid_acc(g[3 * H]) * tanhf(c);
+  const long long o = ((long long)(pos & 1) * L + layer) * n * Hp + (long long)s * Hp + j;
+  h_ring[o] = h;
+  c_ring[o] = c;
+  store_split(out + (long long)s * out_ld + j, out_plane, h);
+}
+
 __global__ void count_active_kernel(const int* __restrict__ active, int n, int* __restrict__ out) {
   __shared__ float red[33];
   float c = 0.f;
@@ -1349,6 +1402,26 @@ int espb_track_scores_f32(const int* parent, const int* tok, const int* bp_paren
   if (n <= 0) return ESPB_OK;
   track_scores_kernel<<<(n + 127) / 128, 128, 0, stream>>>(parent, tok, bp_parent, logp_a, logp_b, V, prev_a, prev_b, new_a, new_b, hist_a, hist_b, step,
                                                           step_ptr, n);
+  ESPB_CHECK_LAUNCH();
+  return ESPB_OK;
+}
+
+int espb_rnnlm_gather_f32(const int* tok, const float* emb, int E, int Ep, const int* anc, int anc_ld, int pos, const int* step_ptr,
+                          const float* h_ring, int L, int n, int H, int Hp, float* xs, cudaStream_t stream) {
+  if (n <= 0) return ESPB_OK;
+  if (E > Ep || H > Hp || (Ep & 3) || (Hp & 3) || L < 1) { espb_set_error("rnnlm_gather: need E <= Ep, H <= Hp, Ep and Hp multiples of 4, L >= 1"); return ESPB_ERR_ARG; }
+  espb::launch_pdl(rnnlm_gather_kernel, dim3(n), dim3(128), 0, stream, tok, emb, E, Ep, anc, anc_ld, pos, step_ptr, h_ring, L, n, H, Hp, xs);
+  ESPB_CHECK_LAUNCH();
+  return ESPB_OK;
+}
+
+int espb_lstm_cell_f32(const float* gates, const int* anc, int anc_ld, int pos, const int* step_ptr, float* h_ring, float* c_ring, int layer, int L,
+                       int n, int H, int Hp, float* out, long long out_plane, int out_ld, cudaStream_t stream) {
+  if (n <= 0) return ESPB_OK;
+  if (H > Hp || layer < 0 || layer >= L || out_ld < H) { espb_set_error("lstm_cell: need H <= Hp, 0 <= layer < L, out_ld >= H"); return ESPB_ERR_ARG; }
+  const long long tot = (long long)n * H;
+  espb::launch_pdl(lstm_cell_kernel, dim3((unsigned)((tot + 255) / 256)), dim3(256), 0, stream, gates, anc, anc_ld, pos, step_ptr, h_ring, c_ring,
+                   layer, L, n, H, Hp, out, out_plane, out_ld);
   ESPB_CHECK_LAUNCH();
   return ESPB_OK;
 }

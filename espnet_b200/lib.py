@@ -77,6 +77,8 @@ _SIGS = {
     "espb_ctc_advance_f32": [P, I, I, I, P, I, I, I, P, P, P, P, P, I, P, P, P, I, P],
     "espb_transpose_tv_f32": [P, I, I, I, P, P],
     "espb_count_active_i32": [P, I, P, P],
+    "espb_rnnlm_gather_f32": [P, P, I, I, P, I, I, P, P, I, I, I, I, P, P],
+    "espb_lstm_cell_f32": [P, P, I, I, P, P, P, I, I, I, I, I, P, L, I, P],
 }
 
 ABI_VERSION = 7   # espb_abi_version() of the library this binding matches (include/espnet_b200.h)

@@ -190,6 +190,17 @@ int espb_axpby_f32(const float* a, float wa, const float* b, float wb, float* ou
 int espb_track_scores_f32(const int* parent, const int* tok, const int* bp_parent, const float* logp_a, const float* logp_b, int V, const float* prev_a,
                           const float* prev_b, float* new_a, float* new_b, float* hist_a, float* hist_b, int step, const int* step_ptr, int n,
                           cudaStream_t stream);
+/* ---- LSTM LM (espnet2/lm/seq_rnn_lm.py:84-166) as a full scorer.  State ring h, c [2][L][n][Hp] fp32: step pos (+ *step_ptr) reads the
+   parent from ring (pos-1)&1 at slot anc[s*anc_ld + pos-1] (zeros at pos 0) and writes ring pos&1 at slot s.  Layer l's GEMM operand is the
+   split [2][n][Kp_l] = [input | parent h] with Kp_0 = Ep + Hp, Kp_l = 2*Hp (l >= 1), the L operands back to back in xs; pad columns are
+   left untouched (the caller zeroes them once). ---- */
+/* embedding row of tok[s] (width E) -> layer 0's input half; parent h of every layer -> that layer's recurrent half */
+int espb_rnnlm_gather_f32(const int* tok, const float* emb, int E, int Ep, const int* anc, int anc_ld, int pos, const int* step_ptr,
+                          const float* h_ring, int L, int n, int H, int Hp, float* xs, cudaStream_t stream);
+/* gates [n][4H] (PyTorch order i, f, g, o) + parent c of layer `layer` -> c' = sig(f) c + sig(i) tanh(g), h' = sig(o) tanh(c') (expf / tanhf)
+   into the ring; h' also split into out[s*out_ld + j] (plane out_plane): the next layer's input half or the output projection's operand */
+int espb_lstm_cell_f32(const float* gates, const int* anc, int anc_ld, int pos, const int* step_ptr, float* h_ring, float* c_ring, int layer, int L,
+                       int n, int H, int Hp, float* out, long long out_plane, int out_ld, cudaStream_t stream);
 int espb_step_inc_i32(int* step, cudaStream_t stream);
 int espb_count_active_i32(const int* active, int n, int* out, cudaStream_t stream);
 
