@@ -673,7 +673,8 @@ __global__ void __launch_bounds__(NW * 32, 16 / NW) dec_src_attn_flash_kernel(co
 
 // ---------------------------------------------------------------- row-wise top-k (descending; ties -> lower index)
 // vals[r][k], ids[r][k] from x[r][0..V) * scale.  One block per row; every thread keeps its V/256 values in registers and the
-// block runs k rounds of arg-max (winner knocked out by its owner).  V <= 256 * NV.
+// block runs k rounds of arg-max (winner knocked out by its owner).  V <= 256 * NV.  Knocked-out entries and columns past V hold
+// NaN, which never compares >=, so genuine -inf entries are still picked (in ascending index order) once the finite ones are used up.
 template <int NV>
 __global__ void __launch_bounds__(256) rows_topk_kernel(const float* __restrict__ x, long long ld, int V, float scale, int k,
                                                         int* __restrict__ ids, float* __restrict__ vals) {
@@ -685,14 +686,14 @@ __global__ void __launch_bounds__(256) rows_topk_kernel(const float* __restrict_
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const int c = threadIdx.x + i * 256;
-    v[i] = (c < V) ? r[c] * scale : -INFINITY;
+    v[i] = (c < V) ? r[c] * scale : __int_as_float(0x7fffffff);
   }
   for (int round = 0; round < k; ++round) {
     float best = -INFINITY; int idx = 0x7fffffff;
 #pragma unroll
-    for (int i = 0; i < NV; ++i) {
+    for (int i = NV - 1; i >= 0; --i) {
       const int c = threadIdx.x + i * 256;
-      if (v[i] > best) { best = v[i]; idx = c; }   // ascending c within a thread: first maximum wins
+      if (v[i] >= best) { best = v[i]; idx = c; }   // descending c within a thread: the last update is the first maximum
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
@@ -713,7 +714,7 @@ __global__ void __launch_bounds__(256) rows_topk_kernel(const float* __restrict_
     __syncthreads();
     const int wi = win_idx;
 #pragma unroll
-    for (int i = 0; i < NV; ++i) if (threadIdx.x + i * 256 == wi) v[i] = -INFINITY;
+    for (int i = 0; i < NV; ++i) if (threadIdx.x + i * 256 == wi) v[i] = __int_as_float(0x7fffffff);
   }
 }
 
@@ -887,8 +888,9 @@ __global__ void __launch_bounds__(NT) beam_select_kernel(BeamState st, int U, in
       if (st.active[s]) {
         if (mode == 1) {
           if (valid[(long long)s * PC + j]) {
-            const float dec = (j < P) ? cand_val[(long long)s * P + j] : w_dec * logp_dec[(long long)s * V + eos];
-            t = ((dec + penalty) + w_ctc * part[(long long)s * PC + j]) + st.score[s];
+            // products rounded on their own (no fma), as the reference's weighted_scores += weight * scores
+            const float dec = (j < P) ? cand_val[(long long)s * P + j] : __fmul_rn(w_dec, logp_dec[(long long)s * V + eos]);
+            t = ((dec + penalty) + __fmul_rn(w_ctc, part[(long long)s * PC + j])) + st.score[s];
           }
         } else {
           t = (cand_val[(long long)s * P + j] + penalty) + st.score[s];
@@ -1190,6 +1192,8 @@ int espb_dec_embed_f32(const int* last_tok, const float* emb, const float* pe, i
 int espb_dec_self_attn_f32(const float* qkv, float* kc, float* vc, const int* anc, int anc_ld, int n, int D, int H, int pos, const int* step_ptr,
                            int max_pos, float* ctx, long long ctx_plane, cudaStream_t stream) {
   const int warps = 4;
+  // lanes hold d = lane + 32 i, i < 4, of a head (dec_self_attn_kernel): wider heads would be silently truncated
+  if (H <= 0 || D % H != 0 || D / H > 128) { espb_set_error("dec_self_attn: needs d_k = D / H an integer <= 128"); return ESPB_ERR_ARG; }
   const int sc_ld = (step_ptr ? max_pos : pos) + 1;   // with a device-side step the score buffer is sized for the longest prefix
   const size_t smem = (size_t)warps * sc_ld * sizeof(float);
   if (smem > 48 * 1024) { espb_set_error("dec_self_attn: prefix too long for the score buffer"); return ESPB_ERR_ARG; }

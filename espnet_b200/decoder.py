@@ -41,6 +41,8 @@ class TransformerDecoder(torch.nn.Module):
         if input_layer != "embed" or not use_output_layer or not normalize_before or concat_after or qk_norm:
             raise NotImplementedError("espnet_b200 TransformerDecoder: embed input, output layer, pre-LN, no concat_after/qk_norm")
         d = encoder_output_size
+        if d // attention_heads > 128:
+            raise NotImplementedError(f"espnet_b200 TransformerDecoder: attention head size <= 128 (got {d} / {attention_heads} heads)")
         self.d, self.heads, self.units, self.num_blocks, self.odim = d, attention_heads, linear_units, num_blocks, vocab_size
         self.embed = torch.nn.Sequential(torch.nn.Embedding(vocab_size, d))
         self.decoders = torch.nn.ModuleList(_DecoderLayer(d, linear_units) for _ in range(num_blocks))

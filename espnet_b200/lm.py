@@ -48,6 +48,8 @@ class TransformerLM(torch.nn.Module):
         super().__init__()
         if pos_enc not in (None, "sinusoidal"):
             raise ValueError(f"unknown pos-enc option: {pos_enc}")
+        if att_unit // head > 128:
+            raise NotImplementedError(f"espnet_b200 TransformerLM: attention head size <= 128 (got {att_unit} / {head} heads)")
         self.vocab_size, self.pos_enc, self.d, self.heads, self.units, self.num_blocks, self.embed_unit = (
             vocab_size, pos_enc, att_unit, head, unit, layer, embed_unit)
         self.embed = torch.nn.Embedding(vocab_size, embed_unit)

@@ -296,12 +296,9 @@ def _ctc_collapse(am, B, Tmax, lens, blank, out_ids, out_len):
 def _rows_topk(x, rows, ld, V, scale, k, ids, vals):
     xv = torch.as_strided(x, (rows, V), (ld, 1), x.storage_offset()) * scale
     for r in range(rows):
-        v = xv[r].clone()
-        for j in range(k):                      # descending, ties -> lower index
-            i = int(torch.argmax(v))            # torch.argmax returns the first maximum
-            ids.view(-1)[r * k + j] = i
-            vals.view(-1)[r * k + j] = v[i]
-            v[i] = float("-inf")
+        i = torch.sort(-xv[r], stable=True).indices[:k]   # descending, ties (-inf included) -> lower index
+        ids.view(-1)[r * k:(r + 1) * k] = i.to(torch.int32)
+        vals.view(-1)[r * k:(r + 1) * k] = xv[r][i]
 
 
 def _dec_embed(last_tok, emb, pe, pos, step_ptr, n, D, scale, x):
@@ -440,6 +437,7 @@ def _beam_select(score, sc_dec, sc_ctc, active, n_score, n_sc_dec, n_sc_ctc, n_a
                  w_dec, w_ctc, penalty, mode, cand_ids, cand_val, logp_dec, part, valid, end_detect, maxlen_cap):
     step += _step(step_ptr)
     f32 = lambda v: float(torch.tensor(v, dtype=torch.float32))  # noqa: E731
+    w_dec, w_ctc, penalty = f32(w_dec), f32(w_ctc), f32(penalty)   # the kernel takes them as float
     PC = P + 1 if mode == 1 else P
     fl = lambda t: t.view(-1)  # noqa: E731
     for u in range(U):

@@ -57,6 +57,18 @@ def _search(model, lm, z, dn):
     return bs, mlr
 
 
+def test_refused_attention_head_size():
+    """The decoder step's self-attention kernel covers heads of up to 128 dimensions: wider heads are refused at construction."""
+    import espnet_b200
+
+    with pytest.raises(NotImplementedError):
+        espnet_b200.lm.TransformerLM(vocab_size=10, att_unit=512, head=2)
+    with pytest.raises(NotImplementedError):
+        espnet_b200.decoder.TransformerDecoder(vocab_size=10, encoder_output_size=512, attention_heads=2, num_blocks=1)
+    espnet_b200.lm.TransformerLM(vocab_size=10, att_unit=512, head=4, layer=1)
+    espnet_b200.decoder.TransformerDecoder(vocab_size=10, encoder_output_size=512, attention_heads=4, num_blocks=1)
+
+
 @pytest.mark.parametrize("dn", DECODES)
 def test_lm_fusion_host_logic_vs_reference_fixture(dn, monkeypatch):
     import emu_backend
