@@ -2,13 +2,19 @@
 // with 128B swizzle), plus a SIMT fp32 GEMM with the same descriptor (validator for the tensor-core path and path for shapes TMA
 // cannot address).
 //
-// Warp roles per CTA (288 threads, one 128 x BN output tile):
-//   warps 0-7: two consumer warpgroups; warpgroup g issues the wgmma for rows [64g, 64g+64) of the tile and runs their epilogue
+// The tensor-core kernel is persistent: min(tiles, SMs) CTAs, CTA c takes 128 x BN output tiles c, c + gridDim.x, ... (see tile_at for
+// the order).  Warp roles per CTA (288 threads):
+//   warps 0-7: two consumer warpgroups; warpgroup g issues the wgmma for rows [64g, 64g+64) of each tile and runs their epilogue
 //              (bias / activation / residual / hi-lo split) straight from the accumulator registers
-//   warp 8   : TMA producer (one elected lane) -> full[s]; the consumers release a stage through empty[s] once its MMAs retired
+//   warp 8   : TMA producer (one elected lane) -> full[s]; the consumers release a stage through empty[s] once its MMAs retired.  The
+//              producer walks the CTA's tiles in the same order, so the next tile's first k-blocks load during the current tile's last
+//              MMAs and its epilogue.
 // The rel-pos band product (EspbGemmDesc::band_t > 0) has its own persistent kernel, relpos_band_kernel.
 #include <cuda.h>
 #include <limits.h>
+
+#include <algorithm>
+#include <cmath>
 #include <stdio.h>
 #include <stdlib.h>
 
@@ -50,12 +56,56 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t adesc, u
   else wgmma_tf32_ss_n64(d, adesc, bdesc, accum);
 }
 
-// Epilogue of two horizontally adjacent accumulator elements (row, col) and (row, col + 1).
-__device__ __forceinline__ void epi_store2(const EpiArgs& e, int row, int col, float v0, float v1, int M, int N, bool vec_ok) {
+// Tile order: batch slices outermost; within a slice the column tiles are walked in bands of `band` column tiles, and within a band the
+// column tile runs fastest.  The CTAs in flight then share a few 128-row blocks of A (each read from HBM about once) and the band's B
+// tiles, which the host sizes to stay in L2 next to the A stream.
+struct TilePos { int m0, n0, bx, by; };
+
+template <int BN>
+__device__ __forceinline__ TilePos tile_at(const EspbGemmDesc& p, long long t, int tiles_m, int tiles_n, int band) {
+  const long long per_slice = (long long)tiles_m * tiles_n;
+  const int z = (int)(t / per_slice);
+  int r = (int)(t - z * per_slice);
+  const int band_tiles = tiles_m * band;
+  const int b = r / band_tiles;
+  r -= b * band_tiles;
+  const int w = min(band, tiles_n - b * band);   // the last band may be narrower
+  TilePos tp;
+  tp.m0 = (r / w) * BM; tp.n0 = (b * band + r % w) * BN; tp.bx = z % p.nbx; tp.by = z / p.nbx;
+  return tp;
+}
+
+// Pair (col, col + 1) of a row of a bias or residual operand; columns past N read as 0.
+__device__ __forceinline__ float2 ld_pair(const float* ptr, int col, int N, bool vec) {
+  if (col + 1 < N) {
+    if (vec) return *reinterpret_cast<const float2*>(ptr + col);
+    return make_float2(ptr[col], ptr[col + 1]);
+  }
+  return make_float2(col < N ? ptr[col] : 0.f, 0.f);
+}
+__device__ __forceinline__ float2 ldg_pair(const float* ptr, int col, int N, bool vec) {
+  if (col + 1 < N) {
+    if (vec) return __ldg(reinterpret_cast<const float2*>(ptr + col));
+    return make_float2(__ldg(ptr + col), __ldg(ptr + col + 1));
+  }
+  return make_float2(col < N ? __ldg(ptr + col) : 0.f, 0.f);
+}
+
+// epi_value with the bias and residual values already loaded.
+__device__ __forceinline__ float epi_apply(const EpiArgs& e, float acc, float b, float r) {
+  float v = acc;
+  if (e.bias) v += b;
+  v = espb::apply_act_acc(v, e.act);
+  v *= e.alpha;
+  if (e.R) v += r;
+  return v;
+}
+
+// Stores two horizontally adjacent epilogue values (row, col) and (row, col + 1).
+__device__ __forceinline__ void epi_store2(const EpiArgs& e, int row, int col, float t0, float t1, int M, int N, bool vec_ok) {
   if (row >= M || col >= N) return;
   float* crow = e.C + (long long)row * e.ldc;
   const bool two = col + 1 < N;
-  const float t0 = epi_value(e, v0, row, col), t1 = two ? epi_value(e, v1, row, col + 1) : 0.f;
   if (vec_ok && two) {
     if (e.split_out) {
       const float h0 = espb::tf32_hi(t0), h1 = espb::tf32_hi(t1);
@@ -73,9 +123,53 @@ __device__ __forceinline__ void epi_store2(const EpiArgs& e, int row, int col, f
   }
 }
 
+// Epilogue of one warpgroup's 64 x BN accumulator tile, in groups of EPI_J 8-column slices.  Each group issues all its bias and residual
+// loads before its first store, so the loads of a group overlap: R is either C itself (each element read and then written by the same
+// thread) or disjoint from C (gemm.h), so no store can feed a load.  With EPI_J = 4 the loaded values, the accumulators and what lives
+// across the out-of-line GELU call fit the 168 registers ptxas gives a thread of this 288-thread CTA; EPI_J = 8 spills.
+constexpr int EPI_J = 4;
+
+template <int BN>
+__device__ __forceinline__ void epilogue(const EspbGemmDesc& p, const TilePos& tp, const float (&d)[BN / 2], int row, int col) {
+  constexpr int G = BN / 8 < EPI_J ? BN / 8 : EPI_J;
+  EpiArgs e;
+  const long long coff = (long long)tp.by * p.sc_y + (long long)tp.bx * p.sc_x;
+  const long long roff = (long long)tp.by * p.sr_y + (long long)tp.bx * p.sr_x;
+  e.C = p.C + coff; e.c_plane = p.c_plane; e.ldc = p.ldc; e.split_out = p.split_out;
+  e.bias = p.bias ? p.bias + (long long)tp.bx * p.sbias_x : nullptr; e.R = p.R ? p.R + roff : nullptr;
+  e.ldr = p.ldr; e.alpha = p.alpha; e.act = p.act;
+  const bool vec_ok = ((p.ldc & 1) == 0) && ((coff & 1) == 0) && ((p.c_plane & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 7) == 0);
+  const bool bias_vec = (reinterpret_cast<uintptr_t>(e.bias) & 7) == 0;
+  const bool r_vec = ((p.ldr & 1) == 0) && ((reinterpret_cast<uintptr_t>(e.R) & 7) == 0);
+#pragma unroll
+  for (int j0 = 0; j0 < BN / 8; j0 += G) {
+    float2 bv[G], rv[G][2];
+#pragma unroll
+    for (int j = 0; j < G; ++j) {
+      const int c = col + 8 * (j0 + j);
+      bv[j] = e.bias ? ldg_pair(e.bias, c, p.N, bias_vec) : make_float2(0.f, 0.f);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = row + 8 * h;
+        rv[j][h] = (e.R && r < p.M) ? ld_pair(e.R + (long long)r * e.ldr, c, p.N, r_vec) : make_float2(0.f, 0.f);
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < G; ++j) {
+      const int i = 4 * (j0 + j);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float t0 = epi_apply(e, d[i + 2 * h], bv[j].x, rv[j][h].x), t1 = epi_apply(e, d[i + 2 * h + 1], bv[j].y, rv[j][h].y);
+        epi_store2(e, row + 8 * h, col + 8 * (j0 + j), t0, t1, p.M, p.N, vec_ok);
+      }
+    }
+  }
+}
+
 template <int BN, int STAGES, bool PROMOTE>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, EspbGemmDesc p, int bxm, int bym, int axm, int aym) {
+gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, EspbGemmDesc p, int bxm, int bym, int axm, int aym,
+                   int tiles_m, int tiles_n, int band) {
   constexpr int B_TILE_BYTES = BN * 128;
   constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
   constexpr int NR = BN / 2;   // accumulator registers per thread: a 64 x BN warpgroup tile over 128 threads
@@ -84,9 +178,8 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   const uint32_t full_bar = smem_base + STAGES * STAGE_BYTES, empty_bar = full_bar + 8 * STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
-  const int bx = blockIdx.z % p.nbx, by = blockIdx.z / p.nbx;
   const int num_kb = (p.K + BK - 1) / BK;
+  const long long ntiles = (long long)tiles_m * tiles_n * p.nbx * p.nby;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 2); }   // empty: one arrival per consumer warpgroup
@@ -101,76 +194,76 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   if (warp == 8) {
     if (elect_one_sync()) {   // one lane, known to ptxas: uniform-datapath issue without per-instruction waterfall loops
       const int cblk = (p.a_mode == 1) ? p.cv_cin / BK : 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        mbar_wait(empty_bar + 8 * s, ph ^ 1);
-        const uint32_t fb = full_bar + 8 * s;
-        mbar_expect_tx(fb, STAGE_BYTES);
-        const uint32_t sa = smem_base + s * STAGE_BYTES;
-        if (p.a_mode == 0) {
-          const int ko = (p.kob > 0) ? kb / p.kob : 0;
-          const int ki = (p.kob > 0) ? kb % p.kob : kb;
-          tma_load_5d(sa, &tmA, fb, ki * BK, m0, bx * axm + ko, by * aym, 0);
-          tma_load_5d(sa + A_TILE_BYTES, &tmA, fb, ki * BK, m0, bx * axm + ko, by * aym, 1);
-        } else {  // conv2: tap (kt,kf) of the 3x3/stride-2 window over the parity-split conv1 output
-          const int tap = kb / cblk, c0 = (kb % cblk) * BK;
-          const int kt = tap / 3, kf = tap % 3;
-          const int par = (kt & 1) * 2 + (kf & 1);
-          tma_load_5d(sa, &tmA, fb, c0, m0 + (kt >> 1), bx + (kf >> 1), par, by);
-          tma_load_5d(sa + A_TILE_BYTES, &tmA, fb, c0, m0 + (kt >> 1), bx + (kf >> 1), 4 + par, by);
+      int s = 0;
+      uint32_t ph = 0;
+      for (long long t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        const TilePos tp = tile_at<BN>(p, t, tiles_m, tiles_n, band);
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(empty_bar + 8 * s, ph ^ 1);
+          const uint32_t fb = full_bar + 8 * s;
+          mbar_expect_tx(fb, STAGE_BYTES);
+          const uint32_t sa = smem_base + s * STAGE_BYTES;
+          if (p.a_mode == 0) {
+            const int ko = (p.kob > 0) ? kb / p.kob : 0;
+            const int ki = (p.kob > 0) ? kb % p.kob : kb;
+            tma_load_5d(sa, &tmA, fb, ki * BK, tp.m0, tp.bx * axm + ko, tp.by * aym, 0);
+            tma_load_5d(sa + A_TILE_BYTES, &tmA, fb, ki * BK, tp.m0, tp.bx * axm + ko, tp.by * aym, 1);
+          } else {  // conv2: tap (kt,kf) of the 3x3/stride-2 window over the parity-split conv1 output
+            const int tap = kb / cblk, c0 = (kb % cblk) * BK;
+            const int kt = tap / 3, kf = tap % 3;
+            const int par = (kt & 1) * 2 + (kf & 1);
+            tma_load_5d(sa, &tmA, fb, c0, tp.m0 + (kt >> 1), tp.bx + (kf >> 1), par, tp.by);
+            tma_load_5d(sa + A_TILE_BYTES, &tmA, fb, c0, tp.m0 + (kt >> 1), tp.bx + (kf >> 1), 4 + par, tp.by);
+          }
+          tma_load_5d(sa + 2 * A_TILE_BYTES, &tmB, fb, kb * BK, tp.n0, tp.bx * bxm, tp.by * bym, 0);
+          tma_load_5d(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, &tmB, fb, kb * BK, tp.n0, tp.bx * bxm, tp.by * bym, 1);
+          if (++s == STAGES) { s = 0; ph ^= 1; }
         }
-        tma_load_5d(sa + 2 * A_TILE_BYTES, &tmB, fb, kb * BK, n0, bx * bxm, by * bym, 0);
-        tma_load_5d(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, &tmB, fb, kb * BK, n0, bx * bxm, by * bym, 1);
       }
     }
     return;
   }
 
   const int wg = warp >> 2;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  const int row_in_tile = wg * 64 + (warp & 3) * 16 + (lane >> 2), col_in_tile = 2 * (lane & 3);
+  int s = 0;
+  uint32_t ph = 0;
   float acc[NR], part[NR];
+  for (long long t = blockIdx.x; t < ntiles; t += gridDim.x) {
+    const TilePos tp = tile_at<BN>(p, t, tiles_m, tiles_n, band);
+    // part is overwritten by the first MMA (scale-d 0); zeroing it here keeps it dead, not live in registers, across the epilogue
 #pragma unroll
-  for (int i = 0; i < NR; ++i) { acc[i] = 0.f; part[i] = 0.f; }
-  for (int kb = 0; kb < num_kb; ++kb) {
-    const int s = kb % STAGES;
-    mbar_wait(full_bar + 8 * s, (kb / STAGES) & 1);
-    const uint32_t sa = smem_base + s * STAGE_BYTES + wg * 64 * 128;   // this warpgroup's 64 rows of A (8 KB: swizzle atoms stay aligned)
-    const uint32_t sb = smem_base + s * STAGE_BYTES + 2 * A_TILE_BYTES;
-    const bool fresh = PROMOTE ? (kb % CHUNK_KB == 0) : (kb == 0);
-    fence_regs(part);
-    wgmma_fence();
+    for (int i = 0; i < NR; ++i) { acc[i] = 0.f; part[i] = 0.f; }
+    // Each k-block's MMAs retire before its stage is released.  Keeping one k-block in flight (wait_group 1) would hold a second stage
+    // per consumer and leave the producer one k-block of lead in the 3-stage ring that fits at BN = 128; measured on H100 that was
+    // slower for long K (conv2: 86 vs 72 ms) and no faster elsewhere.
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(full_bar + 8 * s, ph);   // measured: spinning here gained nothing on the encoder shapes and cost 3 % at M640 N512 K2048
+      const uint32_t sa = smem_base + s * STAGE_BYTES + wg * 64 * 128;   // this warpgroup's 64 rows of A (8 KB: swizzle atoms stay aligned)
+      const uint32_t sb = smem_base + s * STAGE_BYTES + 2 * A_TILE_BYTES;
+      const bool fresh = PROMOTE ? (kb % CHUNK_KB == 0) : (kb == 0);
+      fence_regs(part);
+      wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < BK / 8; ++k) {   // 8 tf32 = 32 bytes per MMA
-      const uint64_t a_hi = gmma_desc(sa + k * 32), a_lo = gmma_desc(sa + A_TILE_BYTES + k * 32);
-      const uint64_t b_hi = gmma_desc(sb + k * 32), b_lo = gmma_desc(sb + B_TILE_BYTES + k * 32);
-      wgmma_tf32<BN>(part, a_lo, b_hi, (fresh && k == 0) ? 0u : 1u);   // small terms first
-      wgmma_tf32<BN>(part, a_hi, b_lo, 1u);
-      wgmma_tf32<BN>(part, a_hi, b_hi, 1u);
+      for (int k = 0; k < BK / 8; ++k) {   // 8 tf32 = 32 bytes per MMA
+        const uint64_t a_hi = gmma_desc(sa + k * 32), a_lo = gmma_desc(sa + A_TILE_BYTES + k * 32);
+        const uint64_t b_hi = gmma_desc(sb + k * 32), b_lo = gmma_desc(sb + B_TILE_BYTES + k * 32);
+        wgmma_tf32<BN>(part, a_lo, b_hi, (fresh && k == 0) ? 0u : 1u);   // small terms first
+        wgmma_tf32<BN>(part, a_hi, b_lo, 1u);
+        wgmma_tf32<BN>(part, a_hi, b_hi, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(part);
+      if (wg_leader) mbar_arrive_local(empty_bar + 8 * s);   // this warpgroup no longer reads the stage
+      if (PROMOTE && (kb % CHUNK_KB == CHUNK_KB - 1 || kb == num_kb - 1)) {
+#pragma unroll
+        for (int i = 0; i < NR; ++i) acc[i] += part[i];
+      }
+      if (++s == STAGES) { s = 0; ph ^= 1; }
     }
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(part);
-    if ((threadIdx.x & 127) == 0) mbar_arrive_local(empty_bar + 8 * s);   // this warpgroup no longer reads the stage
-    if (PROMOTE && (kb % CHUNK_KB == CHUNK_KB - 1 || kb == num_kb - 1)) {
-#pragma unroll
-      for (int i = 0; i < NR; ++i) acc[i] += part[i];
-    }
-  }
-
-  EpiArgs e;
-  const long long coff = (long long)by * p.sc_y + (long long)bx * p.sc_x;
-  const long long roff = (long long)by * p.sr_y + (long long)bx * p.sr_x;
-  e.C = p.C + coff; e.c_plane = p.c_plane; e.ldc = p.ldc; e.split_out = p.split_out;
-  e.bias = p.bias ? p.bias + (long long)bx * p.sbias_x : nullptr; e.R = p.R ? p.R + roff : nullptr;
-  e.ldr = p.ldr; e.alpha = p.alpha; e.act = p.act;
-  const bool vec_ok = ((p.ldc & 1) == 0) && ((coff & 1) == 0) && ((p.c_plane & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 7) == 0);
-  const int row = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
-  const int col = n0 + 2 * (lane & 3);
-#pragma unroll
-  for (int j = 0; j < BN / 8; ++j) {
-    const float* r = PROMOTE ? acc : part;
-    epi_store2(e, row, col + 8 * j, r[4 * j], r[4 * j + 1], p.M, p.N, vec_ok);
-    epi_store2(e, row + 8, col + 8 * j, r[4 * j + 2], r[4 * j + 3], p.M, p.N, vec_ok);
+    epilogue<BN>(p, tp, PROMOTE ? acc : part, tp.m0 + row_in_tile, tp.n0 + col_in_tile);
   }
 }
 
@@ -458,6 +551,39 @@ int make_map(CUtensorMap* map, const float* base, const long long dims[5], const
   return espb_make_tensor_map(map, base, dims, strides_el, BK, box_rows, 1);
 }
 
+int num_sms() {
+  static int n = 0;
+  if (n == 0) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    if (n <= 0) n = 1;
+  }
+  return n;
+}
+
+// B (hi and lo planes) up to GEMM_B_L2_BYTES stays in L2 across the waves of an unbanded walk; larger B is walked in bands of up to
+// GEMM_B_BAND_BYTES.  Measured on H100 (50 MB L2), M = 59968: the CTC head (N 5000, K 512: B = 20 MB) ran 3.25-3.30 ms unbanded against
+// 4.14-4.20 ms in 8 MiB bands; the Transformer's FFN w1 (N 4096, K 1024: B = 32 MB) ran 6.09-6.13 ms in 8 MiB bands against 6.57-6.74
+// unbanded, and 6.28-6.31 ms with 4, 8 or 16 MiB bands.  The threshold lies between those two B sizes.  (The 3.25-3.30 ms CTC head was
+// measured with spinning consumers; with the current waits it runs 4.27-4.47 ms unbanded, as banded: the threshold is neutral there.)
+constexpr long long GEMM_B_L2_BYTES = 24ll << 20;
+constexpr long long GEMM_B_BAND_BYTES = 8ll << 20;
+
+// Column tiles per band (tile_at).  Estimated HBM bytes per batch slice: one band over all columns reads A once, and B once if B stays
+// in L2, else once per wave of SM-count tiles (the CTAs of a wave that share a column tile share its reads).  Narrower bands read A
+// once per band and keep their B in L2.  Bands are used only where that estimate is lower: they pay off for wide B over many row blocks
+// (the Transformer's FFN w1 and CTC head), not where a few row blocks have a long K (conv2, embed.out: A is read per band).
+int column_band(const EspbGemmDesc& d, int bn, int tiles_m, int tiles_n) {
+  const double a_bytes = 2.0 * tiles_m * BM * d.K * sizeof(float), tile_b = 2.0 * bn * d.K * sizeof(float), b_bytes = tiles_n * tile_b;
+  if (b_bytes <= GEMM_B_L2_BYTES) return tiles_n;
+  const int w = (int)std::max(1.0, std::floor(GEMM_B_BAND_BYTES / tile_b));
+  if (w >= tiles_n) return tiles_n;
+  const double waves_per_b = tiles_m / std::max(1.0, (double)num_sms() / tiles_n);
+  const double whole = a_bytes + b_bytes * waves_per_b, banded = a_bytes * ((tiles_n + w - 1) / w) + b_bytes;
+  return banded < whole ? w : tiles_n;
+}
+
 template <int BN, int STAGES, bool PROMOTE>
 int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const EspbGemmDesc& d, int bxm, int bym, int axm, int aym, cudaStream_t stream) {
   constexpr int smem = STAGES * (2 * A_TILE_BYTES + 2 * BN * 128) + 1024 + 16 * STAGES;
@@ -470,22 +596,38 @@ int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const EspbGemmDesc
     }
     attr_set = true;
   }
-  dim3 grid((d.M + BM - 1) / BM, (d.N + BN - 1) / BN, d.nbx * d.nby);
-  if (espb::launch_pdl(gemm_tf32x3_kernel<BN, STAGES, PROMOTE>, grid, dim3(NUM_THREADS), smem, stream, tmA, tmB, d, bxm, bym, axm, aym) != cudaSuccess) {
+  const int tiles_m = (d.M + BM - 1) / BM, tiles_n = (d.N + BN - 1) / BN;
+  const int band = column_band(d, BN, tiles_m, tiles_n);
+  const long long tiles = (long long)tiles_m * tiles_n * d.nbx * d.nby;
+  const int grid = (int)std::min(tiles, (long long)num_sms());
+  if (espb::launch_pdl(gemm_tf32x3_kernel<BN, STAGES, PROMOTE>, dim3(grid), dim3(NUM_THREADS), smem, stream, tmA, tmB, d, bxm, bym, axm, aym, tiles_m,
+                       tiles_n, band) != cudaSuccess) {
     espb_set_error(cudaGetErrorString(cudaGetLastError())); return ESPB_ERR_CUDA;
   }
   return ESPB_OK;
 }
 
-int num_sms() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 1;
+// Lowest and highest byte address of the elements (m, n) of a strided [M, N] window over nbx x nby slices.
+void window_span(const float* base, long long ld, long long sx, long long sy, const EspbGemmDesc& d, uintptr_t& lo, uintptr_t& hi) {
+  long long a = 0, b = (long long)(d.M - 1) * ld + (d.N - 1);
+  const long long ex = (long long)(d.nbx - 1) * sx, ey = (long long)(d.nby - 1) * sy;
+  (ex < 0 ? a : b) += ex;
+  (ey < 0 ? a : b) += ey;
+  lo = reinterpret_cast<uintptr_t>(base + a);
+  hi = reinterpret_cast<uintptr_t>(base + b) + sizeof(float) - 1;
+}
+
+// The epilogue contract of gemm.h: R is C itself or shares no address range with what the GEMM writes.
+bool residual_ok(const EspbGemmDesc& d) {
+  if (!d.R) return true;
+  if (d.R == d.C && d.ldr == d.ldc && d.sr_x == d.sc_x && d.sr_y == d.sc_y) return true;
+  uintptr_t rlo, rhi, clo, chi;
+  window_span(d.R, d.ldr, d.sr_x, d.sr_y, d, rlo, rhi);
+  for (int plane = 0; plane < (d.split_out ? 2 : 1); ++plane) {
+    window_span(d.C + plane * d.c_plane, d.ldc, d.sc_x, d.sc_y, d, clo, chi);
+    if (rlo <= chi && clo <= rhi) return false;
   }
-  return n;
+  return true;
 }
 
 template <int NKB, bool PROMOTE>
@@ -569,6 +711,7 @@ int espb_make_tensor_map(CUtensorMap* map, const float* base, const long long di
 
 int espb_gemm_tc_launch(const EspbGemmDesc& d, cudaStream_t stream, int version) {
   if (d.M <= 0 || d.N <= 0 || d.K <= 0 || d.nbx <= 0 || d.nby <= 0) { espb_set_error("gemm: bad shape"); return ESPB_ERR_ARG; }
+  if (!residual_ok(d)) { espb_set_error("gemm: residual R partially overlaps the output C"); return ESPB_ERR_ARG; }
   CUtensorMap tmA, tmB;
   int rc;
   int axm = 1, aym = 1;
@@ -623,6 +766,7 @@ int espb_gemm_tc_launch(const EspbGemmDesc& d, cudaStream_t stream, int version)
 
 int espb_gemm_simt_launch(const EspbGemmDesc& d, cudaStream_t stream) {
   if (d.M <= 0 || d.N <= 0 || d.K <= 0 || d.nbx <= 0 || d.nby <= 0) { espb_set_error("gemm: bad shape"); return ESPB_ERR_ARG; }
+  if (!residual_ok(d)) { espb_set_error("gemm: residual R partially overlaps the output C"); return ESPB_ERR_ARG; }
   dim3 grid((d.M + 63) / 64, (d.N + 63) / 64, d.nbx * d.nby);
   gemm_simt_kernel<<<grid, 256, 0, stream>>>(d);
   ESPB_CHECK_LAUNCH();

@@ -21,7 +21,10 @@ struct EspbGemmDesc {
   int split_out;        // 1: write hi/lo planes (c_plane apart); 0: plain fp32
   const float* bias;    // [N] or null
   long long sbias_x;    // bias offset per batch-x index (heads as batch: bias + bx*sbias_x)
-  const float* R; long long ldr, sr_x, sr_y;            // residual (may alias C) or null
+  const float* R; long long ldr, sr_x, sr_y;            // residual or null: either C itself (R == C, ldr == ldc, sr_* == sc_*: in place)
+                                                        //   or sharing no address with the C window (both planes with split_out); a
+                                                        //   tensor-core thread loads all its R elements before its first store, so the
+                                                        //   launch refuses a partial overlap with ESPB_ERR_ARG
   float alpha;          // out = R + alpha * act(acc + bias)   (R absent: alpha * act(...))
   int act;              // espb::ACT_*
   int cv_t1h, cv_f1h, cv_cin;  // mode 1: conv1-output half extents and channel count
