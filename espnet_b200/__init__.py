@@ -3,12 +3,13 @@
 Public surface mirrors the reference classes on that path (see SURVEY.md section 8b):
 Speech2Text, ESPnetASRModel, DefaultFrontend, UtteranceMVN, ConformerEncoder, CTC,
 TransformerDecoder, BatchBeamSearch, Hypothesis, TooShortUttError (+ GlobalMVN, the output-side text classes, and the
-TransformerEncoder of the next scope row and the EBranchformerEncoder; CTCPrefixScorer and TransformerDecoder.batch_score implement the reference's scorer protocol,
+TransformerEncoder of the next scope row, the EBranchformerEncoder and the BranchformerEncoder; CTCPrefixScorer and TransformerDecoder.batch_score implement the reference's scorer protocol,
 ``espnet_b200.integration.register()`` adds the classes to the reference's registries).
 All compute goes through the C-ABI CUDA library ``libespnet_b200.so`` (include/espnet_b200.h).
 """
 from .asr_inference import (ESPnetASRModel, Speech2Text, build_model, build_model_from_file, decoder_choices,  # noqa: F401
                             encoder_choices, frontend_choices, normalize_choices)
+from .branchformer_encoder import BranchformerEncoder  # noqa: F401
 from .ctc import CTC, CTCPrefixScorer  # noqa: F401
 from .decoder import TransformerDecoder  # noqa: F401
 from .e_branchformer_encoder import EBranchformerEncoder  # noqa: F401

@@ -18,6 +18,7 @@ import torch
 import yaml
 
 from . import lib
+from .branchformer_encoder import BranchformerEncoder
 from .ctc import CTC
 from .decoder import TransformerDecoder
 from .e_branchformer_encoder import EBranchformerEncoder
@@ -36,7 +37,7 @@ normalize_choices = {"global_mvn": GlobalMVN, "utterance_mvn": UtteranceMVN}
 from .streaming_encoder import ContextualBlockConformerEncoder  # noqa: E402
 
 encoder_choices = {"conformer": ConformerEncoder, "transformer": TransformerEncoder, "contextual_block_conformer": ContextualBlockConformerEncoder,
-                   "e_branchformer": EBranchformerEncoder}
+                   "e_branchformer": EBranchformerEncoder, "branchformer": BranchformerEncoder}
 decoder_choices = {"transformer": TransformerDecoder}
 
 
@@ -73,7 +74,11 @@ def build_model(args: argparse.Namespace) -> ESPnetASRModel:
     """ASRTask.build_model (espnet2/tasks/asr.py:512-651) for the supported classes."""
     token_list = list(args.token_list)
     vocab_size = len(token_list)
-    for key in ("specaug", "preencoder", "postencoder"):
+    # SpecAug (specaug: specaug) augments only in training (espnet_model.py:394) and has no parameters or buffers: every recipe-written
+    # config.yaml names it, so it is accepted and specaug_conf ignored
+    if getattr(args, "specaug", None) not in (None, "specaug"):
+        raise NotImplementedError(f"specaug={args.specaug} is not on the espnet_b200 inference path")
+    for key in ("preencoder", "postencoder"):
         if getattr(args, key, None) is not None:
             raise NotImplementedError(f"{key} is not on the espnet_b200 inference path")
     if getattr(args, "input_size", None) is not None:

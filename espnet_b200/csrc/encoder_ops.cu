@@ -1,6 +1,7 @@
 // Warp-primitive kernels of the Conformer encoder: LayerNorm, conv1 of the 2-D subsampling, rel-pos
 // attention glue (q+u / q+v, V transpose, rel-shift + masked softmax) and the convolution module's
-// GLU + depthwise conv + BatchNorm(eval) + Swish, and the E-Branchformer's cgMLP gating unit and merge module.  All outputs that feed a GEMM are written as
+// GLU + depthwise conv + BatchNorm(eval) + Swish, the E-Branchformer's cgMLP gating unit and merge module, and the Branchformer's
+// learned / fixed branch averaging.  All outputs that feed a GEMM are written as
 // tf32 hi/lo planes (see gemm.h).
 //
 // Reference: espnet2/legacy/nets/pytorch_backend/transformer/{layer_norm,subsampling,attention}.py,
@@ -605,6 +606,111 @@ __global__ void gather_rows_kernel(const float* __restrict__ src, long long src_
   for (int d = threadIdx.x; d < D; d += blockDim.x) o[d] = s[d];
 }
 
+// ---------------------------------------------------------------- Branchformer merge (branchformer_encoder.py:206-276)
+// learned_ave weights of utterance b: per branch k, s_t = (x_t . pool_w[k] + pool_b[k]) / sqrt(D) over the rows t < lens[b];
+// pooled = sum_t softmax_t(s)_t x_t; weight_k = pooled . wt_w[k] + wt_b[k]; merge_w[b] = softmax(weight_0, weight_1).
+// Pass 1 reads every valid row of both branches once: block (chunk, b, k) writes the online-softmax partials of its BP_ROWS rows -- the
+// max m, l = sum exp(s - m) and acc = sum exp(s - m) x_t -- to part[b][k][chunk][D + 2].  Pass 2 (one block per utterance) rescales the
+// partials to the common max, divides by the total and finishes both dot products and the 2-way softmax on the device.
+constexpr int BP_ROWS = 32;
+constexpr int BP_THREADS = 256;
+
+__global__ void __launch_bounds__(BP_THREADS) branch_pool_partial_kernel(const float* __restrict__ x1, const float* __restrict__ x2, long long ldx,
+                                                                         int Tmax, int D, const int* __restrict__ lens,
+                                                                         const float* __restrict__ pool_w, const float* __restrict__ pool_b,
+                                                                         int nchunk, float* __restrict__ part) {
+  const int c = blockIdx.x, b = blockIdx.y, k = blockIdx.z;
+  const int t0 = c * BP_ROWS, len = lens[b];
+  if (t0 >= len) return;
+  const int nrows = min(BP_ROWS, len - t0);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const float* x = (k ? x2 : x1) + ((long long)b * Tmax + t0) * ldx;
+  const float* wp = pool_w + (long long)k * D;
+  __shared__ float s[BP_ROWS], p[BP_ROWS];
+  const float sq = sqrtf((float)D);
+  for (int r = warp; r < nrows; r += BP_THREADS / 32) {   // one warp per row: the pooling score
+    const float* xr = x + (long long)r * ldx;
+    float a = 0.f;
+    for (int d = lane; d < D; d += 32) a = fmaf(xr[d], wp[d], a);
+    a = espb::warp_sum(a);
+    if (lane == 0) s[r] = (a + pool_b[k]) / sq;
+  }
+  __syncthreads();
+  float* out = part + (((long long)b * 2 + k) * nchunk + c) * (D + 2);
+  if (warp == 0) {   // BP_ROWS == 32: one score per lane
+    const float sv = lane < nrows ? s[lane] : -INFINITY;
+    const float m = espb::warp_max(sv);
+    const float e = lane < nrows ? expf(sv - m) : 0.f;
+    const float l = espb::warp_sum(e);
+    p[lane] = e;
+    if (lane == 0) { out[0] = m; out[1] = l; }
+  }
+  __syncthreads();
+  for (int d = threadIdx.x; d < D; d += BP_THREADS) {   // the rows are still in L1 / L2
+    float a = 0.f;
+    for (int r = 0; r < nrows; ++r) a = fmaf(p[r], x[(long long)r * ldx + d], a);
+    out[2 + d] = a;
+  }
+}
+
+__global__ void __launch_bounds__(BP_THREADS) branch_pool_combine_kernel(const int* __restrict__ lens, int D, const float* __restrict__ wt_w,
+                                                                         const float* __restrict__ wt_b, int nchunk, const float* __restrict__ part,
+                                                                         float* __restrict__ merge_w) {
+  const int b = blockIdx.x;
+  const int nc = min(nchunk, (max(lens[b], 0) + BP_ROWS - 1) / BP_ROWS);
+  __shared__ float red[33];
+  float wgt[2];
+  for (int k = 0; k < 2; ++k) {
+    const float* pk = part + ((long long)b * 2 + k) * nchunk * (D + 2);
+    float m = -INFINITY, l = 0.f;
+    for (int c = 0; c < nc; ++c) m = fmaxf(m, pk[(long long)c * (D + 2)]);
+    for (int c = 0; c < nc; ++c) l += pk[(long long)c * (D + 2) + 1] * expf(pk[(long long)c * (D + 2)] - m);
+    const float inv = l > 0.f ? 1.f / l : 0.f;   // no valid row (lens[b] == 0): pooled = 0
+    float dot = 0.f;
+    for (int d = threadIdx.x; d < D; d += BP_THREADS) {
+      float a = 0.f;
+      for (int c = 0; c < nc; ++c) a = fmaf(pk[(long long)c * (D + 2) + 2 + d], expf(pk[(long long)c * (D + 2)] - m), a);
+      dot = fmaf(a * inv, wt_w[(long long)k * D + d], dot);
+    }
+    wgt[k] = espb::block_sum(dot, red) + wt_b[k];
+  }
+  if (threadIdx.x == 0) {
+    const float mx = fmaxf(wgt[0], wgt[1]);
+    const float e0 = expf(wgt[0] - mx), e1 = expf(wgt[1] - mx);
+    merge_w[2 * b] = e0 / (e0 + e1);
+    merge_w[2 * b + 1] = e1 / (e0 + e1);
+  }
+}
+
+// out = split(w1 * x1 + w2 * x2) [M][D], four columns per thread: (w1, w2) = merge_w[row / Tmax][0..1], or the constants c1 / c2 when merge_w
+// is null.  Both products are rounded before the add (no FMA contraction), as torch evaluates w1 * x1 + w2 * x2.
+__global__ void __launch_bounds__(256) branch_merge_kernel(const float* __restrict__ x1, const float* __restrict__ x2, long long ldx, long long M,
+                                                           int D, int Tmax, const float* __restrict__ merge_w, float c1, float c2,
+                                                           float* __restrict__ out, long long plane) {
+  const int D4 = D >> 2;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= M * D4) return;
+  const long long r = i / D4;
+  const int col = (int)(i - r * D4) * 4;
+  float w1 = c1, w2 = c2;
+  if (merge_w) {
+    const long long b = r / Tmax;
+    w1 = merge_w[2 * b];
+    w2 = merge_w[2 * b + 1];
+  }
+  const float4 a = *reinterpret_cast<const float4*>(x1 + r * ldx + col);
+  const float4 e = *reinterpret_cast<const float4*>(x2 + r * ldx + col);
+  float4 y;
+  y.x = __fadd_rn(__fmul_rn(w1, a.x), __fmul_rn(w2, e.x));
+  y.y = __fadd_rn(__fmul_rn(w1, a.y), __fmul_rn(w2, e.y));
+  y.z = __fadd_rn(__fmul_rn(w1, a.z), __fmul_rn(w2, e.z));
+  y.w = __fadd_rn(__fmul_rn(w1, a.w), __fmul_rn(w2, e.w));
+  const float4 h = make_float4(tf32_hi(y.x), tf32_hi(y.y), tf32_hi(y.z), tf32_hi(y.w));
+  const float4 lo = make_float4(tf32_lo(y.x, h.x), tf32_lo(y.y, h.y), tf32_lo(y.z, h.z), tf32_lo(y.w, h.w));
+  *reinterpret_cast<float4*>(out + r * D + col) = h;
+  *reinterpret_cast<float4*>(out + plane + r * D + col) = lo;
+}
+
 }  // namespace
 
 extern "C" {
@@ -772,6 +878,32 @@ int espb_merge_dwconv_f32(const float* cat, int B, int Tmax, int C2, const int* 
   if (K == 3) dwconv_tile_kernel<3, false><<<grid, 256, smem, stream>>>(cat, C2, 0, Tmax, C2, lens, nullptr, nullptr, nullptr, w, b, K, out, out_plane);
   else if (K == 31) dwconv_tile_kernel<31, false><<<grid, 256, smem, stream>>>(cat, C2, 0, Tmax, C2, lens, nullptr, nullptr, nullptr, w, b, K, out, out_plane);
   else dwconv_tile_kernel<0, false><<<grid, 256, smem, stream>>>(cat, C2, 0, Tmax, C2, lens, nullptr, nullptr, nullptr, w, b, K, out, out_plane);
+  ESPB_CHECK_LAUNCH();
+  return ESPB_OK;
+}
+
+int espb_branch_pool_f32(const float* x1, const float* x2, long long ldx, int B, int Tmax, int D, const int* lens, const float* pool_w,
+                         const float* pool_b, const float* weight_w, const float* weight_b, float* part, float* merge_w, cudaStream_t stream) {
+  if (D <= 0 || ldx < D) { espb_set_error("branch_pool: need 0 < D <= ldx"); return ESPB_ERR_ARG; }
+  if (B <= 0 || Tmax <= 0) return ESPB_OK;
+  const int nchunk = (Tmax + BP_ROWS - 1) / BP_ROWS;
+  branch_pool_partial_kernel<<<dim3(nchunk, B, 2), BP_THREADS, 0, stream>>>(x1, x2, ldx, Tmax, D, lens, pool_w, pool_b, nchunk, part);
+  ESPB_CHECK_LAUNCH();
+  branch_pool_combine_kernel<<<B, BP_THREADS, 0, stream>>>(lens, D, weight_w, weight_b, nchunk, part, merge_w);
+  ESPB_CHECK_LAUNCH();
+  return ESPB_OK;
+}
+
+int espb_branch_merge_f32(const float* x1, const float* x2, long long ldx, long long M, int D, int Tmax, const float* merge_w, float w1, float w2,
+                          float* out, long long out_plane, cudaStream_t stream) {
+  const uintptr_t al = reinterpret_cast<uintptr_t>(x1) | reinterpret_cast<uintptr_t>(x2) | reinterpret_cast<uintptr_t>(out);
+  if (D <= 0 || (D & 3) || (ldx & 3) || ldx < D || (out_plane & 3) || (al & 15) || Tmax <= 0) {
+    espb_set_error("branch_merge: need D, ldx and out_plane multiples of 4, 16-byte aligned x1 / x2 / out, ldx >= D and Tmax > 0");
+    return ESPB_ERR_ARG;
+  }
+  if (M <= 0) return ESPB_OK;
+  const long long n4 = M * (D / 4);
+  branch_merge_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, stream>>>(x1, x2, ldx, M, D, Tmax, merge_w, w1, w2, out, out_plane);
   ESPB_CHECK_LAUNCH();
   return ESPB_OK;
 }

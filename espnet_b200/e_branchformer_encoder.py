@@ -3,7 +3,7 @@
 Reference: espnet2/asr/encoder/e_branchformer_encoder.py:55-563 (EBranchformerEncoderLayer, EBranchformerEncoder) and
 espnet2/asr/layers/cgmlp.py:15-124 (ConvolutionalSpatialGatingUnit, ConvolutionalGatingMLP).  The subsampling, the FFNs and the attention
 branch are the shared ones of layers.py -- the Conformer's rel-pos "latest" self-attention (band GEMM over a cached P_all, then the fused
-wgmma attention at d_k = 64); the cgMLP branch is
+wgmma attention at d_k = 64); the cgMLP branch, shared with the Branchformer in layers.py, is
 channel_proj1 with GELU in the GEMM epilogue, the CSGU kernel (LayerNorm + depthwise conv + gating, csrc/encoder_ops.cu) and
 channel_proj2; the merge module is one depthwise-conv kernel over the concatenated branches followed by merge_proj.
 
@@ -16,28 +16,12 @@ from typing import List, Optional, Tuple
 
 import torch
 
-from .layers import LN_EPS, EncoderBase, _FFN, _PosBias
+from .layers import LN_EPS, EncoderBase, _CgMLP, _FFN, _PosBias
 # new_split stays importable here although _pos in layers.py allocates: the kernel emulation of the tests replaces it in this module
 from .lib import call, ptr
 from .ops import ACT_GELU, ACT_RELU, ACT_SWISH, _count, gemm, layernorm, linear, new_split, split_from  # noqa: F401
 
 _FFN_ACTS = {"swish": ACT_SWISH, "relu": ACT_RELU}   # get_activation (nets_utils.py:571-584) choices this path computes
-
-
-class _CSGU(torch.nn.Module):
-    def __init__(self, size, kernel_size):
-        super().__init__()
-        n = size // 2
-        self.norm = torch.nn.LayerNorm(n, eps=LN_EPS)
-        self.conv = torch.nn.Conv1d(n, n, kernel_size, 1, (kernel_size - 1) // 2, groups=n)
-
-
-class _CgMLP(torch.nn.Module):
-    def __init__(self, size, units, kernel_size):
-        super().__init__()
-        self.channel_proj1 = torch.nn.Sequential(torch.nn.Linear(size, units), torch.nn.GELU())
-        self.csgu = _CSGU(units, kernel_size)
-        self.channel_proj2 = torch.nn.Linear(units // 2, size)
 
 
 class _Layer(torch.nn.Module):
@@ -100,17 +84,13 @@ class EBranchformerEncoder(EncoderBase):
         f32, ln, D = self._f32, self._pack_ln, self._output_size
         layers = []
         for lyr in self.encoders:
-            cg = lyr.cgmlp
             d = dict(norm_mha=ln(lyr.norm_mha), norm_mlp=ln(lyr.norm_mlp), norm_final=ln(lyr.norm_final))
             if self.use_ffn:
                 d["norm_ff"], d["ffn"] = ln(lyr.norm_ff), self._pack_ffn(lyr.feed_forward)
             if self.macaron:
                 d["norm_ff_macaron"], d["ffn_macaron"] = ln(lyr.norm_ff_macaron), self._pack_ffn(lyr.feed_forward_macaron)
             d.update(self._pack_mha(lyr.attn))
-            d["p1_w"], d["p1_b"] = split_from(f32(cg.channel_proj1[0].weight)), f32(cg.channel_proj1[0].bias)
-            d["csgu_ln"] = ln(cg.csgu.norm)
-            d["csgu_w"], d["csgu_b"] = f32(cg.csgu.conv.weight).view(self.cgmlp_units // 2, -1), f32(cg.csgu.conv.bias)
-            d["p2_w"], d["p2_b"] = split_from(f32(cg.channel_proj2.weight)), f32(cg.channel_proj2.bias)
+            d.update(self._pack_cgmlp(lyr.cgmlp))
             d["mg_w"], d["mg_b"] = f32(lyr.depthwise_conv_fusion.weight).view(2 * D, -1), f32(lyr.depthwise_conv_fusion.bias)
             d["mp_w"], d["mp_b"] = split_from(f32(lyr.merge_proj.weight)), f32(lyr.merge_proj.bias)
             layers.append(d)
@@ -129,8 +109,8 @@ class EBranchformerEncoder(EncoderBase):
         keys, own conv boundaries in the CSGU and the merge module); rows t >= olens[b] of the output are 0."""
         pk = self._packed or self._pack()
         xs_pad, T, olens, lens32 = self._lengths(xs_pad, ilens)   # check_short_utt: e_branchformer_encoder.py:482-499
-        B, D, U = xs_pad.shape[0], self._output_size, self.cgmlp_units
-        M, Uh = B * T, U // 2
+        B, D = xs_pad.shape[0], self._output_size
+        M = B * T
         x = self._buf("x", (M, D))
         self._subsample(xs_pad, x, math.sqrt(D))
         if self.trace is not None:
@@ -138,9 +118,6 @@ class EBranchformerEncoder(EncoderBase):
         p_all = self._pos(T)
 
         xn, qkv, ctx = self._buf("xn", (2, M, D)), self._buf("qkv", (2, M, 3 * D)), self._buf("ctx", (2, M, D))
-        g1 = self._buf("g1", (M, U))              # channel_proj1 + GELU, plain
-        stats = self._buf("stats", (M, 2))        # CSGU LayerNorm mean / rstd per row
-        g2 = self._buf("g2", (2, M, Uh))          # CSGU output, split
         cat = self._buf("cat", (M, 2 * D))        # [x_att | x_cgmlp], plain
         mg = self._buf("mg", (2, M, 2 * D))       # cat + dwconv(cat), split
         for li, w in enumerate(pk["layers"]):
@@ -152,12 +129,7 @@ class EBranchformerEncoder(EncoderBase):
             self._relpos_attn(qkv, w, li, p_all, ctx, B, T, lens32)
             gemm(M, D, D, ctx, M * D, D, w["out_w"], D * D, D, cat, 2 * D, bias=w["out_b"])
             # branch 2: cgMLP (e_branchformer_encoder.py:154-163, cgmlp.py:110-124) -> cat[:, D:]
-            layernorm(x, *w["norm_mlp"], LN_EPS, out_split=xn)
-            linear(xn, w["p1_w"], g1, bias=w["p1_b"], act=ACT_GELU)
-            call("espb_csgu_f32", ptr(g1), B, T, U, ptr(lens32), ptr(w["csgu_ln"][0]), ptr(w["csgu_ln"][1]), LN_EPS, ptr(w["csgu_w"]),
-                 ptr(w["csgu_b"]), self.cgmlp_kernel, ptr(stats), ptr(g2), M * Uh)
-            _count(2)
-            gemm(M, D, Uh, g2, M * Uh, Uh, w["p2_w"], D * Uh, Uh, cat, 2 * D, bias=w["p2_b"], c_off=D)
+            self._cgmlp(x, xn, w, B, T, lens32, cat, 2 * D, c_off=D)
             # merge: x += merge_proj(cat + dwconv(cat))  (e_branchformer_encoder.py:165-170)
             call("espb_merge_dwconv_f32", ptr(cat), B, T, 2 * D, ptr(lens32), ptr(w["mg_w"]), ptr(w["mg_b"]), self.merge_kernel, ptr(mg), M * 2 * D)
             _count()

@@ -13,7 +13,8 @@ import espnet_b200
 NAMES = {"frontend": {"b200_default": "DefaultFrontend"},
          "normalize": {"b200_utterance_mvn": "UtteranceMVN", "b200_global_mvn": "GlobalMVN"},
          "encoder": {"b200_conformer": "ConformerEncoder", "b200_transformer": "TransformerEncoder",
-                     "b200_contextual_block_conformer": "ContextualBlockConformerEncoder", "b200_e_branchformer": "EBranchformerEncoder"},
+                     "b200_contextual_block_conformer": "ContextualBlockConformerEncoder", "b200_e_branchformer": "EBranchformerEncoder",
+                     "b200_branchformer": "BranchformerEncoder"},
          "decoder": {"b200_transformer": "TransformerDecoder"}}
 
 

@@ -12,7 +12,7 @@ import torch
 
 from . import ops
 from .errors import TooShortUttError
-from .ops import ACT_RELU, _count, layernorm, linear, split_from
+from .ops import ACT_GELU, ACT_RELU, _count, layernorm, linear, split_from
 
 # Launches go through ops.call / ops.ptr / ops.gemm / ops.new_split, looked up at call time: the kernel emulation of the tests
 # (tests/emu_backend.py) replaces them in ops and in each encoder module.
@@ -59,6 +59,24 @@ class _ConvModule(torch.nn.Module):
         self.depthwise_conv = torch.nn.Conv1d(channels, channels, kernel_size, padding=(kernel_size - 1) // 2, groups=channels)
         self.norm = torch.nn.BatchNorm1d(channels)
         self.pointwise_conv2 = torch.nn.Conv1d(channels, channels, 1)
+
+
+class _CSGU(torch.nn.Module):
+    def __init__(self, size, kernel_size):
+        super().__init__()
+        n = size // 2
+        self.norm = torch.nn.LayerNorm(n, eps=LN_EPS)
+        self.conv = torch.nn.Conv1d(n, n, kernel_size, 1, (kernel_size - 1) // 2, groups=n)
+
+
+class _CgMLP(torch.nn.Module):
+    """ConvolutionalGatingMLP (cgmlp.py:84-124) with the identity gate and no linear after the conv."""
+
+    def __init__(self, size, units, kernel_size):
+        super().__init__()
+        self.channel_proj1 = torch.nn.Sequential(torch.nn.Linear(size, units), torch.nn.GELU())
+        self.csgu = _CSGU(units, kernel_size)
+        self.channel_proj2 = torch.nn.Linear(units // 2, size)
 
 
 class _Conv2dSubsampling(torch.nn.Module):
@@ -161,8 +179,16 @@ class EncoderBase(torch.nn.Module):
         return d
 
     def _pack_pos(self, attns):
-        """linear_pos of every layer stacked [L*D][D]: one GEMM per length projects the rel-pos table for all layers (_pos)."""
+        """linear_pos of every attention layer stacked [L*D][D], L = the number of attention layers (layer ordinal a at rows a*D..): one GEMM
+        per length projects the rel-pos table for all of them (_pos)."""
         return split_from(torch.cat([self._f32(a.linear_pos.weight) for a in attns], 0))
+
+    def _pack_cgmlp(self, cg):
+        """channel_proj1, the CSGU's LayerNorm and depthwise conv, channel_proj2 of a _CgMLP."""
+        f32 = self._f32
+        return dict(p1_w=split_from(f32(cg.channel_proj1[0].weight)), p1_b=f32(cg.channel_proj1[0].bias), csgu_ln=self._pack_ln(cg.csgu.norm),
+                    csgu_w=f32(cg.csgu.conv.weight).view(cg.csgu.conv.weight.shape[0], -1), csgu_b=f32(cg.csgu.conv.bias),
+                    p2_w=split_from(f32(cg.channel_proj2.weight)), p2_b=f32(cg.channel_proj2.bias))
 
     def _pack_conv(self, cm):
         f32, D = self._f32, self._output_size
@@ -243,23 +269,43 @@ class EncoderBase(torch.nn.Module):
         _count()
         linear(cv, w["pw2_w"], x, bias=w["pw2_b"], residual=x)
 
+    def _cgmlp(self, x, xn, w, B, T, lens32, out, ldc, c_off=0, split_out=False, residual=None):
+        """ConvolutionalGatingMLP(norm_mlp(x)) (cgmlp.py:110-124) of the M = B*T rows of x into out[:, c_off:c_off + D] (row stride ldc; a
+        split out has planes of M*ldc), plus residual when given: norm_mlp, channel_proj1 with GELU in the epilogue, the CSGU kernel
+        (LayerNorm + depthwise conv + gating, each utterance seeing zeros outside its own rows), channel_proj2."""
+        D, U, K = self._output_size, self.cgmlp_units, self.cgmlp_kernel
+        M, Uh = B * T, U // 2
+        g1 = self._buf("g1", (M, U))              # channel_proj1 + GELU, plain
+        stats = self._buf("stats", (M, 2))        # CSGU LayerNorm mean / rstd per row
+        g2 = self._buf("g2", (2, M, Uh))          # CSGU output, split
+        layernorm(x, *w["norm_mlp"], LN_EPS, out_split=xn)
+        linear(xn, w["p1_w"], g1, bias=w["p1_b"], act=ACT_GELU)
+        ops.call("espb_csgu_f32", ops.ptr(g1), B, T, U, ops.ptr(lens32), ops.ptr(w["csgu_ln"][0]), ops.ptr(w["csgu_ln"][1]), LN_EPS,
+                 ops.ptr(w["csgu_w"]), ops.ptr(w["csgu_b"]), K, ops.ptr(stats), ops.ptr(g2), M * Uh)
+        _count(2)
+        ops.gemm(M, D, Uh, g2, M * Uh, Uh, w["p2_w"], D * Uh, Uh, out, ldc, c_plane=M * ldc if split_out else 0, split_out=split_out,
+                 bias=w["p2_b"], R=residual, ldr=D if residual is not None else 0, c_off=c_off)
+
     def _pos(self, T):
-        """P_all split [2][2T-1][L*D] = linear_pos(pos_emb) for every layer (one GEMM per length, cached)."""
+        """P_all split [2][2T-1][L*D] = linear_pos(pos_emb) for every attention layer (one GEMM per length, cached); L*D is the width of
+        the packed pos_w_all."""
         if T not in self._pos_cache:
             if len(self._pos_cache) > 8:
                 self._pos_cache.clear()
-            D, L = self._output_size, self.num_blocks
+            D, LD = self._output_size, self._packed["pos_w_all"].shape[1]
             pe = split_from(rel_pos_table(T, D).to(self.after_norm.weight.device))
-            out = ops.new_split(2 * T - 1, L * D, device=pe.device)
+            out = ops.new_split(2 * T - 1, LD, device=pe.device)
             linear(pe, self._packed["pos_w_all"], out, split_out=True)
             self._pos_cache[T] = out
         return self._pos_cache[T]
 
     def _relpos_attn(self, qkv, w, li, p_all, ctx, B, T, lens32):
-        """RelPositionMultiHeadedAttention (attention.py:416-459) of layer li, from the fused q|k|v projection qkv (split [2][B*T][3D]) to
-        ctx (split [2][B*T][D]); the output projection is the caller's.  p_all = _pos(T)."""
-        D, H, L = self._output_size, self.heads, self.num_blocks
+        """RelPositionMultiHeadedAttention (attention.py:416-459) of attention layer li (its ordinal among the layers with attention, which
+        is the layer index in an encoder where every layer has one), from the fused q|k|v projection qkv (split [2][B*T][3D]) to ctx (split
+        [2][B*T][D]); the output projection is the caller's.  p_all = _pos(T)."""
+        D, H = self._output_size, self.heads
         dk, M, R = D // H, B * T, 2 * T - 1
+        L = p_all.shape[2] // D
         Tp, Rp = _pitch(T), _pitch(R)
         qu, qv = self._buf("qu", (2, M, D)), self._buf("qv", (2, M, D))
         vt = self._buf("vt", (2, B, H, dk, Tp))

@@ -52,6 +52,8 @@ _SIGS = {
     "espb_zero_pad_rows_f32": [P, I, I, I, P, L, I, P],
     "espb_csgu_f32": [P, I, I, I, P, P, P, F, P, P, I, P, P, L, P],
     "espb_merge_dwconv_f32": [P, I, I, I, P, P, P, I, P, L, P],
+    "espb_branch_pool_f32": [P, P, L, I, I, I, P, P, P, P, P, P, P, P],
+    "espb_branch_merge_f32": [P, P, L, L, I, I, P, F, F, P, L, P],
     "espb_cbe_build_chunks_f32": [P, I, I, I, I, I, I, P, I, I, F, P, P, P, P],
     "espb_cbe_ctx_propagate_f32": [P, I, I, I, I, P, P, I, I, P],
     "espb_zero_rows_f32": [P, L, L, L, I, L, I, P],

@@ -119,6 +119,18 @@ int espb_csgu_f32(const float* h, int B, int Tmax, int U, const int* lens, const
  * depthwise over C2 channels with zeros outside [0, lens[b]); rows t >= lens[b] of out are 0.  w [C2][K], K odd <= 127. */
 int espb_merge_dwconv_f32(const float* cat, int B, int Tmax, int C2, const int* lens, const float* w, const float* b, int K, float* out,
                           long long out_plane, cudaStream_t stream);
+/* Branchformer learned_ave merge weights (branchformer_encoder.py:221-266): x1 / x2 [B][Tmax] rows of D floats at row stride ldx (plain).
+ * For branch k of utterance b, over its rows t < lens[b] only: s_t = (x_t . pool_w[k] + pool_b[k]) / sqrt(D), p = softmax_t(s),
+ * weight_k = (sum_t p_t x_t) . weight_w[k] + weight_b[k]; merge_w[b][0..1] = softmax(weight_0, weight_1).  pool_w / weight_w [2][D],
+ * pool_b / weight_b [2].  One read of the rows (online softmax over 32-row chunks, then a combine launch); no host synchronisation.
+ * part: caller workspace of B * 2 * ceil(Tmax / 32) * (D + 2) floats. */
+int espb_branch_pool_f32(const float* x1, const float* x2, long long ldx, int B, int Tmax, int D, const int* lens, const float* pool_w,
+                         const float* pool_b, const float* weight_w, const float* weight_b, float* part, float* merge_w, cudaStream_t stream);
+/* Branchformer weighted branch average (branchformer_encoder.py:268-276): out = split(w1 * x1 + w2 * x2) [M][D], each product rounded before
+ * the add.  (w1, w2) = merge_w[row / Tmax][0..1] (espb_branch_pool_f32), or the constants w1 / w2 when merge_w is NULL (fixed_ave).  x1 / x2
+ * rows at stride ldx; D, ldx and out_plane multiples of 4, x1 / x2 / out 16-byte aligned. */
+int espb_branch_merge_f32(const float* x1, const float* x2, long long ldx, long long M, int D, int Tmax, const float* merge_w, float w1, float w2,
+                          float* out, long long out_plane, cudaStream_t stream);
 
 /* ---- streaming encoder: contextual block processing (espnet2/asr/encoder/contextual_block_conformer_encoder.py:506-572,
  *      legacy/nets/pytorch_backend/conformer/contextual_block_encoder_layer.py:291-308) ---- */
