@@ -44,6 +44,7 @@ int espb_device_sm(int* major, int* minor) {
 // use_tc = 1: wgmma 3xTF32 kernel, 2: the same with chunked fp32 promotion (TMA needs 16-byte aligned strides/bases); 0: SIMT fp32 kernel.
 int espb_gemm_f32(const EspbGemmDesc* d, int use_tc, cudaStream_t stream) {
   if (!d) { espb_set_error("gemm: null descriptor"); return ESPB_ERR_ARG; }
+  if (d->a_mode < 0 || d->a_mode > 3) { espb_set_error("gemm: a_mode must be 0..3"); return ESPB_ERR_ARG; }
   return use_tc ? espb_gemm_tc_launch(*d, stream, use_tc == 2 ? 2 : 1) : espb_gemm_simt_launch(*d, stream);
 }
 

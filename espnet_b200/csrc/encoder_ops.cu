@@ -125,38 +125,58 @@ __global__ void split_kernel(const float* __restrict__ x, long long n, float* __
 }
 
 // ---------------------------------------------------------------- conv1: Conv2d(1, C, 3, stride 2) + ReLU (subsampling.py:400-402)
-// feats [B][Tf_max][F] -> parity-split NHWC planes [B][plane*4 + (t1&1)*2 + (f1&1)][F1h][T1h][C]
-// (hi/lo planes), the layout conv2's implicit GEMM reads with unit-stride TMA boxes.
+// feats [B][Tf_max][F] -> NHWC planes split into the s*s phases of the next conv's stride s,
+// [B][plane*s*s + (t1%s)*s + (f1%s)][F1h][T1h][C] (hi/lo planes, F1h = ceil(F1/s), T1h = ceil(T1/s)): the layout the implicit-GEMM conv
+// that follows reads with unit-stride TMA boxes (gemm.h: conv_geom).
 __global__ void __launch_bounds__(256) conv1_relu_kernel(const float* __restrict__ feats, int Tf_max, int F, const float* __restrict__ w /*[C][9]*/,
-                                                         const float* __restrict__ bias, int C, float* __restrict__ out, int T1, int F1, int T1h,
-                                                         int F1h) {
+                                                         const float* __restrict__ bias, int C, float* __restrict__ out, int T1, int F1, int s,
+                                                         int T1h, int F1h) {
   extern __shared__ float rows[];  // 3 * F input rows
   const int b = blockIdx.y, t1 = blockIdx.x;
   const float* in = feats + ((long long)b * Tf_max + 2 * t1) * F;
   for (int i = threadIdx.x; i < 3 * F; i += blockDim.x) rows[i] = in[i];
   __syncthreads();
   const long long sub = (long long)F1h * T1h * C;
-  float* ob = out + (long long)b * 8 * sub;
-  const int pt = t1 & 1, tt = t1 >> 1;
+  const int nph = s * s;
+  float* ob = out + (long long)b * 2 * nph * sub;
+  const int pt = t1 % s, tt = t1 / s;
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     float wk[9];
 #pragma unroll
     for (int i = 0; i < 9; ++i) wk[i] = w[c * 9 + i];
     const float bc = bias[c];
-    for (int f1 = 0; f1 < F1; ++f1) {
+    for (int f1 = 0, pf = 0, ff = 0; f1 < F1; ++f1) {   // f1 = ff * s + pf
       float acc = bc;
 #pragma unroll
       for (int kt = 0; kt < 3; ++kt)
 #pragma unroll
         for (int kf = 0; kf < 3; ++kf) acc = fmaf(rows[kt * F + 2 * f1 + kf], wk[kt * 3 + kf], acc);
       acc = fmaxf(acc, 0.f);
-      const int par = pt * 2 + (f1 & 1), ff = f1 >> 1;
-      float* o = ob + par * sub + ((long long)ff * T1h + tt) * C + c;
+      float* o = ob + (pt * s + pf) * sub + ((long long)ff * T1h + tt) * C + c;
       float h = tf32_hi(acc);
       o[0] = h;
-      o[4 * sub] = tf32_lo(acc, h);
+      o[nph * sub] = tf32_lo(acc, h);
+      if (++pf == s) { pf = 0; ++ff; }
     }
   }
+}
+
+// ---------------------------------------------------------------- conv output -> phase-split input of the next strided conv
+// x split [B][F][T][C] (hi/lo planes x_plane apart) -> [B][plane*s*s + (t%s)*s + (f%s)][Fh][Th][C]; C a multiple of 4, 16-byte aligned.
+__global__ void phase_split_kernel(const float4* __restrict__ x, long long x_plane4, int F, int T, int C4, int s, int Th, int Fh,
+                                   float4* __restrict__ out, long long rows) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= rows * C4) return;
+  const int c = (int)(i % C4);
+  const long long r = i / C4;
+  const int t = (int)(r % T);
+  const long long bf = r / T;
+  const int f = (int)(bf % F), b = (int)(bf / F);
+  const int nph = s * s;
+  const long long sub = (long long)Fh * Th * C4;
+  float4* o = out + (long long)b * 2 * nph * sub + ((t % s) * s + f % s) * sub + ((long long)(f / s) * Th + t / s) * C4 + c;
+  o[0] = x[i];
+  o[nph * sub] = x[i + x_plane4];
 }
 
 // ---------------------------------------------------------------- attention glue (attention.py:416-459)
@@ -779,11 +799,31 @@ int espb_split_tf32_f32(const float* x, long long n, float* out, long long plane
   return ESPB_OK;
 }
 
+int espb_conv1_relu_phase_f32(const float* feats, int B, int Tf_max, int F, const float* w, const float* bias, int C, float* out, int T1, int F1,
+                              int s, int T1h, int F1h, cudaStream_t stream) {
+  if (T1 <= 0 || F1 <= 0) { espb_set_error("conv1: empty output"); return ESPB_ERR_ARG; }
+  if (s < 1 || s > 3 || T1h * s < T1 || F1h * s < F1) { espb_set_error("conv1: phase stride s must be 1..3 with s * T1h >= T1, s * F1h >= F1"); return ESPB_ERR_ARG; }
+  dim3 grid(T1, B);
+  conv1_relu_kernel<<<grid, 256, 3 * F * sizeof(float), stream>>>(feats, Tf_max, F, w, bias, C, out, T1, F1, s, T1h, F1h);
+  ESPB_CHECK_LAUNCH();
+  return ESPB_OK;
+}
+
 int espb_conv1_relu_f32(const float* feats, int B, int Tf_max, int F, const float* w, const float* bias, int C, float* out, int T1, int F1,
                         int T1h, int F1h, cudaStream_t stream) {
-  if (T1 <= 0 || F1 <= 0) { espb_set_error("conv1: empty output"); return ESPB_ERR_ARG; }
-  dim3 grid(T1, B);
-  conv1_relu_kernel<<<grid, 256, 3 * F * sizeof(float), stream>>>(feats, Tf_max, F, w, bias, C, out, T1, F1, T1h, F1h);
+  return espb_conv1_relu_phase_f32(feats, B, Tf_max, F, w, bias, C, out, T1, F1, 2, T1h, F1h, stream);
+}
+
+int espb_phase_split_f32(const float* x, long long x_plane, int B, int F, int T, int C, int s, int Th, int Fh, float* out, cudaStream_t stream) {
+  if (B <= 0 || F <= 0 || T <= 0) return ESPB_OK;
+  if (s < 1 || s > 3 || Th * s < T || Fh * s < F) { espb_set_error("phase split: s must be 1..3 with s * Th >= T, s * Fh >= F"); return ESPB_ERR_ARG; }
+  if (C % 4 || x_plane % 4 || (reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(out) & 15)) {
+    espb_set_error("phase split: C and x_plane must be multiples of 4, x and out 16-byte aligned");
+    return ESPB_ERR_ARG;
+  }
+  const long long rows = (long long)B * F * T, n = rows * (C / 4);
+  phase_split_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const float4*>(x), x_plane / 4, F, T, C / 4, s, Th, Fh,
+                                                                      reinterpret_cast<float4*>(out), rows);
   ESPB_CHECK_LAUNCH();
   return ESPB_OK;
 }

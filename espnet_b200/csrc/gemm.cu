@@ -193,7 +193,8 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
 
   if (warp == 8) {
     if (elect_one_sync()) {   // one lane, known to ptxas: uniform-datapath issue without per-instruction waterfall loops
-      const int cblk = (p.a_mode == 1) ? p.cv_cin / BK : 0;
+      const int cblk = (p.a_mode != 0) ? p.cv_cin / BK : 0;
+      const ConvGeom g = conv_geom(p.a_mode);
       int s = 0;
       uint32_t ph = 0;
       for (long long t = blockIdx.x; t < ntiles; t += gridDim.x) {
@@ -208,12 +209,12 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
             const int ki = (p.kob > 0) ? kb % p.kob : kb;
             tma_load_5d(sa, &tmA, fb, ki * BK, tp.m0, tp.bx * axm + ko, tp.by * aym, 0);
             tma_load_5d(sa + A_TILE_BYTES, &tmA, fb, ki * BK, tp.m0, tp.bx * axm + ko, tp.by * aym, 1);
-          } else {  // conv2: tap (kt,kf) of the 3x3/stride-2 window over the parity-split conv1 output
+          } else {  // conv: tap (kt,kf) of the k x k / stride-s window over the phase-split input (conv_geom)
             const int tap = kb / cblk, c0 = (kb % cblk) * BK;
-            const int kt = tap / 3, kf = tap % 3;
-            const int par = (kt & 1) * 2 + (kf & 1);
-            tma_load_5d(sa, &tmA, fb, c0, tp.m0 + (kt >> 1), tp.bx + (kf >> 1), par, tp.by);
-            tma_load_5d(sa + A_TILE_BYTES, &tmA, fb, c0, tp.m0 + (kt >> 1), tp.bx + (kf >> 1), 4 + par, tp.by);
+            const int kt = tap / g.k, kf = tap - kt * g.k;
+            const int par = (kt % g.s) * g.s + kf % g.s;
+            tma_load_5d(sa, &tmA, fb, c0, tp.m0 + kt / g.s, tp.bx + kf / g.s, par, tp.by);
+            tma_load_5d(sa + A_TILE_BYTES, &tmA, fb, c0, tp.m0 + kt / g.s, tp.bx + kf / g.s, g.s * g.s + par, tp.by);
           }
           tma_load_5d(sa + 2 * A_TILE_BYTES, &tmB, fb, kb * BK, tp.n0, tp.bx * bxm, tp.by * bym, 0);
           tma_load_5d(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, &tmB, fb, kb * BK, tp.n0, tp.bx * bxm, tp.by * bym, 1);
@@ -487,14 +488,15 @@ __device__ __forceinline__ float load_a(const EspbGemmDesc& p, int bx, int by, i
     off = (long long)by * p.sa_y + (long long)(bx + ko) * p.sa_x + (long long)m * p.lda + ki;
     return p.A[off] + p.A[off + p.a_plane];
   }
-  // conv2 over [b][plane*4 + pt*2 + pf][F1h][T1h][C]
-  const int tap = k / p.cv_cin, c = k % p.cv_cin, kt = tap / 3, kf = tap % 3;
-  const int par = (kt & 1) * 2 + (kf & 1);
-  const int tt = m + (kt >> 1), ff = bx + (kf >> 1);
+  // conv over [b][plane*s*s + pt*s + pf][F_in/s][T_in/s][C] (conv_geom)
+  const ConvGeom g = conv_geom(p.a_mode);
+  const int tap = k / p.cv_cin, c = k % p.cv_cin, kt = tap / g.k, kf = tap % g.k;
+  const int par = (kt % g.s) * g.s + kf % g.s, nph = g.s * g.s;
+  const int tt = m + kt / g.s, ff = bx + kf / g.s;
   if (tt >= p.cv_t1h || ff >= p.cv_f1h) return 0.f;
   const long long sub = (long long)p.cv_f1h * p.cv_t1h * p.cv_cin;
-  off = (long long)by * 8 * sub + ((long long)ff * p.cv_t1h + tt) * p.cv_cin + c;
-  return p.A[off + par * sub] + p.A[off + (4 + par) * sub];
+  off = (long long)by * 2 * nph * sub + ((long long)ff * p.cv_t1h + tt) * p.cv_cin + c;
+  return p.A[off + par * sub] + p.A[off + (nph + par) * sub];
 }
 __device__ __forceinline__ float load_b(const EspbGemmDesc& p, int bx, int by, int n, int k) {
   if (n >= p.N || k >= p.K) return 0.f;
@@ -724,10 +726,14 @@ int espb_gemm_tc_launch(const EspbGemmDesc& d, cudaStream_t stream, int version)
     long long str[4] = {d.lda, d.sa_x, d.sa_y, d.a_plane};
     rc = make_map(&tmA, d.A, dims, str, BM);
   } else {
-    if (d.cv_cin % BK != 0 || d.K != 9 * d.cv_cin) { espb_set_error("conv2 gemm: cin must be a multiple of 32"); return ESPB_ERR_ARG; }
-    const long long sub = (long long)d.cv_f1h * d.cv_t1h * d.cv_cin;
-    long long dims[5] = {d.cv_cin, d.cv_t1h, d.cv_f1h, 8, d.nby};
-    long long str[4] = {d.cv_cin, (long long)d.cv_t1h * d.cv_cin, sub, 8 * sub};
+    const ConvGeom g = conv_geom(d.a_mode);
+    if (d.cv_cin % BK != 0 || d.K != g.k * g.k * d.cv_cin) {
+      espb_set_error("conv gemm: cin must be a multiple of 32 and K = k*k*cin");
+      return ESPB_ERR_ARG;
+    }
+    const long long sub = (long long)d.cv_f1h * d.cv_t1h * d.cv_cin, nph = g.s * g.s;
+    long long dims[5] = {d.cv_cin, d.cv_t1h, d.cv_f1h, 2 * nph, d.nby};
+    long long str[4] = {d.cv_cin, (long long)d.cv_t1h * d.cv_cin, sub, 2 * nph * sub};
     rc = make_map(&tmA, d.A, dims, str, BM);
   }
   if (rc != ESPB_OK) return rc;

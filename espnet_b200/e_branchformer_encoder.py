@@ -16,7 +16,7 @@ from typing import List, Optional, Tuple
 
 import torch
 
-from .layers import LN_EPS, EncoderBase, _CgMLP, _FFN, _PosBias
+from .layers import LN_EPS, SUBSAMPLING, EncoderBase, _CgMLP, _FFN, _PosBias
 # new_split stays importable here although _pos in layers.py allocates: the kernel emulation of the tests replaces it in this module
 from .lib import call, ptr
 from .ops import ACT_GELU, ACT_RELU, ACT_SWISH, _count, gemm, layernorm, linear, new_split, split_from  # noqa: F401
@@ -55,7 +55,7 @@ class EBranchformerEncoder(EncoderBase):
                  interctc_use_conditioning: bool = False, qk_norm: bool = False, use_flash_attn: bool = True,
                  gradient_checkpoint_layers: List[int] = []):
         unsupported = []
-        if input_layer != "conv2d": unsupported.append(f"input_layer={input_layer}")
+        if input_layer not in SUBSAMPLING: unsupported.append(f"input_layer={input_layer}")
         if rel_pos_type != "latest" or pos_enc_layer_type != "rel_pos" or attention_layer_type != "rel_selfattn":
             unsupported.append("rel_pos_type/pos_enc_layer_type/attention_layer_type other than latest/rel_pos/rel_selfattn")
         if use_linear_after_conv or gate_activation != "identity": unsupported.append("use_linear_after_conv / non-identity gate_activation")
@@ -72,7 +72,7 @@ class EBranchformerEncoder(EncoderBase):
             raise NotImplementedError("espnet_b200 EBranchformerEncoder: output_size must be a multiple of 32")
         super().__init__(input_size, output_size, (
             _Layer(output_size, attention_heads, cgmlp_linear_units, cgmlp_conv_kernel, linear_units, use_ffn, macaron_ffn, merge_conv_kernel)
-            for _ in range(num_blocks)))
+            for _ in range(num_blocks)), input_layer)
         self.heads, self.num_blocks = attention_heads, num_blocks
         self.cgmlp_units, self.cgmlp_kernel, self.merge_kernel = cgmlp_linear_units, cgmlp_conv_kernel, merge_conv_kernel
         self.use_ffn, self.macaron = use_ffn, use_ffn and macaron_ffn

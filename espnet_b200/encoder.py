@@ -4,7 +4,7 @@ CUDA kernels (wgmma 3xTF32 GEMMs + warp-primitive glue).
 Reference: espnet2/asr/encoder/conformer_encoder.py:89-429 and the legacy modules it composes
 (Conv2dSubsampling, RelPositionalEncoding, EncoderLayer, RelPositionMultiHeadedAttention,
 PositionwiseFeedForward, ConvolutionModule, LayerNorm).  Supported configuration = the one
-BASELINE.json names: input_layer "conv2d", rel_pos_type "latest" (rel_pos / rel_selfattn),
+BASELINE.json names, with input_layer "conv2d", "conv2d2", "conv2d6" or "conv2d8"; rel_pos_type "latest" (rel_pos / rel_selfattn),
 macaron_style, use_cnn_module, swish, normalize_before, no intermediate CTC.  The subsampling, FFN,
 rel-pos self-attention and convolution module are the shared ones of layers.py.  The torch.nn layers
 are parameter containers only (so that reference checkpoints load by name); forward never calls them.
@@ -14,7 +14,7 @@ from typing import List, Optional, Tuple, Union
 
 import torch
 
-from .layers import LN_EPS, EncoderBase, _ConvModule, _FFN, _PosBias
+from .layers import LN_EPS, SUBSAMPLING, EncoderBase, _ConvModule, _FFN, _PosBias
 # call / ptr / gemm / new_split stay importable here although the shared code in layers.py launches: the kernel emulation of the
 # tests replaces these names in every encoder module
 from .lib import call, ptr  # noqa: F401
@@ -49,7 +49,7 @@ class ConformerEncoder(EncoderBase):
                  stochastic_depth_rate: Union[float, List[float]] = 0.0, layer_drop_rate: float = 0.0,
                  max_pos_emb_len: int = 5000, qk_norm: bool = False, use_flash_attn: bool = True):
         unsupported = []
-        if input_layer != "conv2d": unsupported.append(f"input_layer={input_layer}")
+        if input_layer not in SUBSAMPLING: unsupported.append(f"input_layer={input_layer}")
         if rel_pos_type != "latest" or pos_enc_layer_type != "rel_pos" or selfattention_layer_type != "rel_selfattn":
             unsupported.append("rel_pos_type/pos_enc_layer_type/selfattention_layer_type other than latest/rel_pos/rel_selfattn")
         if not (normalize_before and macaron_style and use_cnn_module) or concat_after: unsupported.append("non pre-LN macaron+cnn block")
@@ -61,7 +61,7 @@ class ConformerEncoder(EncoderBase):
         if output_size % 32:
             raise NotImplementedError("espnet_b200 ConformerEncoder: output_size must be a multiple of 32")
         super().__init__(input_size, output_size,
-                         (_EncoderLayer(output_size, attention_heads, linear_units, cnn_module_kernel) for _ in range(num_blocks)))
+                         (_EncoderLayer(output_size, attention_heads, linear_units, cnn_module_kernel) for _ in range(num_blocks)), input_layer)
         self.heads, self.num_blocks, self.kernel = attention_heads, num_blocks, cnn_module_kernel
 
     def _pack(self):

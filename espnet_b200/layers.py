@@ -79,14 +79,24 @@ class _CgMLP(torch.nn.Module):
         self.channel_proj2 = torch.nn.Linear(units // 2, size)
 
 
-class _Conv2dSubsampling(torch.nn.Module):
-    """Conv2dSubsampling and Conv2dSubsamplingWOPosEnc: the same parameters (the positional encoding has none)."""
+# input_layer -> (kernel, stride) of the convs after the first Conv2d(1, odim, 3, 2) (subsampling.py:386-860), and check_short_utt's limit
+# (subsampling.py:31-48): the fewest input frames that leave one output frame.
+SUBSAMPLING = {"conv2d": ((3, 2),), "conv2d2": ((3, 1),), "conv2d6": ((5, 3),), "conv2d8": ((3, 2), (3, 2))}
+MIN_FRAMES = {"conv2d": 7, "conv2d2": 7, "conv2d6": 11, "conv2d8": 15}
+_A_MODE = {(3, 2): 1, (3, 1): 2, (5, 3): 3}   # (kernel, stride) -> EspbGemmDesc.a_mode of the implicit-GEMM conv (gemm.h: conv_geom)
 
-    def __init__(self, idim, odim):
+
+class _Conv2dSubsampling(torch.nn.Module):
+    """Conv2dSubsampling{,2,6,8} and Conv2dSubsamplingWOPosEnc: conv.0 / conv.2 (/ conv.4) and out, sized by the input layer (the
+    positional encoding has no parameters)."""
+
+    def __init__(self, idim, odim, input_layer="conv2d"):
         super().__init__()
-        self.conv = torch.nn.Sequential(torch.nn.Conv2d(1, odim, 3, 2), torch.nn.ReLU(), torch.nn.Conv2d(odim, odim, 3, 2),
-                                        torch.nn.ReLU())
-        self.out = torch.nn.Linear(odim * (((idim - 1) // 2 - 1) // 2), odim)
+        convs = [torch.nn.Conv2d(1, odim, 3, 2), torch.nn.ReLU()]
+        for k, s in SUBSAMPLING[input_layer]:
+            convs += [torch.nn.Conv2d(odim, odim, k, s), torch.nn.ReLU()]
+        self.conv = torch.nn.Sequential(*convs)
+        self.out = torch.nn.Linear(odim * subsampled_len(idim, input_layer)[-1], odim)
 
 
 def _sinusoid_table(pos, d):
@@ -110,10 +120,12 @@ def rel_pos_table(T, d):
     return _sinusoid_table(torch.arange(T - 1, -T, -1, dtype=torch.float32), d)
 
 
-def subsampled_len(n):
-    """Lengths after the two 3x3 stride-2 convs of Conv2dSubsampling: (after conv1, after conv2)."""
-    n1 = (n - 3) // 2 + 1
-    return n1, (n1 - 3) // 2 + 1
+def subsampled_len(n, input_layer="conv2d"):
+    """Lengths after each conv of the input layer's subsampling (after conv1, after conv2[, after conv3]); n an int or an integer tensor."""
+    out = [(n - 3) // 2 + 1]
+    for k, s in SUBSAMPLING[input_layer]:
+        out.append((out[-1] - k) // s + 1)
+    return tuple(out)
 
 
 def _pitch(n):
@@ -130,10 +142,10 @@ class EncoderBase(torch.nn.Module):
     trace = None            # set to a list to collect per-stage outputs (tests)
     last_split_out = None   # split copy of the last output (feeds the CTC head / decoder memory GEMMs)
 
-    def __init__(self, input_size, output_size, layers):
+    def __init__(self, input_size, output_size, layers, input_layer="conv2d"):
         super().__init__()
-        self._output_size, self.idim = output_size, input_size
-        self.embed = _Conv2dSubsampling(input_size, output_size)
+        self._output_size, self.idim, self.input_layer = output_size, input_size, input_layer
+        self.embed = _Conv2dSubsampling(input_size, output_size, input_layer)
         self.encoders = torch.nn.ModuleList(layers)
         self.after_norm = torch.nn.LayerNorm(output_size, eps=LN_EPS)
         self._packed, self._ws = None, {}
@@ -202,52 +214,74 @@ class EncoderBase(torch.nn.Module):
         return d
 
     def _pack_io(self):
-        """Conv2dSubsampling in the layouts of the conv1 kernel and the implicit-GEMM conv2, and after_norm."""
+        """Conv2dSubsampling in the layouts of the conv1 kernel and the implicit-GEMM convs, and after_norm."""
         f32, e = self._f32, self.embed
         D = C = self._output_size
-        F1, F2 = subsampled_len(self.idim)
-        return dict(F1=F1, F2=F2, c1_w=f32(e.conv[0].weight).view(C, 9), c1_b=f32(e.conv[0].bias),
-                    # conv2 weight [co][ci][kt][kf] -> [co][(kt*3+kf)*C + ci]
-                    c2_w=split_from(f32(e.conv[2].weight).permute(0, 2, 3, 1).reshape(C, 9 * C)), c2_b=f32(e.conv[2].bias),
-                    # embed.out columns are c*F2+f (subsampling.py:450-451) -> f*C+c to match the [B][F2][T][C] conv2 output
-                    out_w=split_from(f32(e.out.weight).view(D, C, F2).permute(0, 2, 1).reshape(D, F2 * C)), out_b=f32(e.out.bias),
+        Fs = subsampled_len(self.idim, self.input_layer)
+        convs = []
+        for i, (k, _) in enumerate(SUBSAMPLING[self.input_layer]):
+            # weight [co][ci][kt][kf] -> [co][(kt*k+kf)*C + ci]
+            cv = e.conv[2 * i + 2]
+            convs.append((split_from(f32(cv.weight).permute(0, 2, 3, 1).reshape(C, k * k * C)), f32(cv.bias)))
+        return dict(F=Fs, c1_w=f32(e.conv[0].weight).view(C, 9), c1_b=f32(e.conv[0].bias), convs=convs,
+                    # embed.out columns are c*F+f (subsampling.py:450-451) -> f*C+c to match the [B][F][T][C] output of the last conv
+                    out_w=split_from(f32(e.out.weight).view(D, C, Fs[-1]).permute(0, 2, 1).reshape(D, Fs[-1] * C)), out_b=f32(e.out.bias),
                     after_norm=self._pack_ln(self.after_norm))
 
     # ---------------------------------------------------------------- launches
     def _lengths(self, xs_pad, ilens):
-        """check_short_utt (subsampling.py:43-44) and the subsampled lengths -> (xs_pad fp32 contiguous, T, olens, lens32 on the device).
+        """check_short_utt (subsampling.py:31-48) and the subsampled lengths -> (xs_pad fp32 contiguous, T, olens, lens32 on the device).
 
         The reference decodes one utterance per call, so the limit applies to every utterance of a ragged batch, not to the padded length
-        (an utterance with < 7 frames would get olens 0)."""
+        (an utterance below the limit would get olens 0)."""
         xs_pad = xs_pad.contiguous().float()
         B, Tf, F = xs_pad.shape
         assert F == self.idim
+        lim = MIN_FRAMES[self.input_layer]
         min_len = int(torch.as_tensor(ilens).min()) if torch.as_tensor(ilens).numel() else Tf
-        if Tf < 7 or min_len < 7:
+        if Tf < lim or min_len < lim:
             size = min(Tf, min_len)
-            which = "" if Tf < 7 else f" (utterance {int(torch.as_tensor(ilens).argmin())} of the batch)"
-            raise TooShortUttError(f"has {size} frames and is too short for subsampling (it needs more than 7 frames), "
-                                   f"return empty results{which}", size, 7)
-        olens = torch.div(torch.div(ilens - 1, 2, rounding_mode="trunc") - 1, 2, rounding_mode="trunc")
-        return xs_pad, subsampled_len(Tf)[1], olens, olens.to(device=xs_pad.device, dtype=torch.int32).contiguous()
+            which = "" if Tf < lim else f" (utterance {int(torch.as_tensor(ilens).argmin())} of the batch)"
+            raise TooShortUttError(f"has {size} frames and is too short for subsampling (it needs more than {lim} frames), "
+                                   f"return empty results{which}", size, lim)
+        olens = subsampled_len(torch.as_tensor(ilens), self.input_layer)[-1]
+        return xs_pad, subsampled_len(Tf, self.input_layer)[-1], olens, olens.to(device=xs_pad.device, dtype=torch.int32).contiguous()
 
     def _subsample(self, xs, x, alpha, pe=None):
-        """Conv2dSubsampling (subsampling.py:432-474) of xs (B, T_f, idim) into x [B*T][D]: x = alpha * out(conv(xs)) [+ pe[t]], the
-        positional table entering as a batch-broadcast residual of the embed.out GEMM."""
+        """Conv2dSubsampling{,2,6,8} (subsampling.py:432-474, 625-649, 730-754, 838-862) of xs (B, T_f, idim) into x [B*T][D]:
+        x = alpha * out(conv(xs)) [+ pe[t]], the positional table entering as a batch-broadcast residual of the embed.out GEMM.
+
+        conv1 writes its output split into the phases of the next conv's stride; each following conv is an implicit GEMM over such a
+        phase-split input (one output frequency per batch x slice), and its split [B][F][T][C] output is re-laid into phases when another
+        strided conv follows (conv2d8)."""
         pk = self._packed
         B, Tf, F = xs.shape
         D = C = self._output_size
-        F1, F2 = pk["F1"], pk["F2"]
-        T1, T = subsampled_len(Tf)
-        T1h, F1h = (T1 + 1) // 2, (F1 + 1) // 2
-        c1 = self._buf("c1", (B, 8, F1h, T1h, C), zero=True)
-        ops.call("espb_conv1_relu_f32", ops.ptr(xs), B, Tf, F, ops.ptr(pk["c1_w"]), ops.ptr(pk["c1_b"]), C, ops.ptr(c1), T1, F1, T1h, F1h)
+        geo = SUBSAMPLING[self.input_layer]
+        Fs, Ts = pk["F"], subsampled_len(Tf, self.input_layer)
+        s = geo[0][1]
+        Th, Fh = -(-Ts[0] // s), -(-Fs[0] // s)
+        a = self._buf("c1", (B, 2 * s * s, Fh, Th, C), zero=True)
+        if s == 2:   # the parity split (conv2d, conv2d8): the s = 2 entry point of the same kernel
+            ops.call("espb_conv1_relu_f32", ops.ptr(xs), B, Tf, F, ops.ptr(pk["c1_w"]), ops.ptr(pk["c1_b"]), C, ops.ptr(a), Ts[0], Fs[0], Th, Fh)
+        else:
+            ops.call("espb_conv1_relu_phase_f32", ops.ptr(xs), B, Tf, F, ops.ptr(pk["c1_w"]), ops.ptr(pk["c1_b"]), C, ops.ptr(a), Ts[0], Fs[0],
+                     s, Th, Fh)
         _count()
-        c2 = self._buf("c2", (2, B, F2, T, C))
-        ops.gemm(T, C, 9 * C, c1, 0, 0, pk["c2_w"], C * 9 * C, 9 * C, c2, C, c_plane=B * F2 * T * C, split_out=True, bias=pk["c2_b"],
-                 act=ACT_RELU, nbx=F2, nby=B, sc=(T * C, F2 * T * C), a_mode=1, conv=(T1h, F1h, C))
-        ops.gemm(T, D, F2 * C, c2, B * F2 * T * C, C, pk["out_w"], D * F2 * C, F2 * C, x, D, bias=pk["out_b"], alpha=alpha, R=pe,
-                 ldr=0 if pe is None else D, nbx=1, nby=B, sa=(T * C, F2 * T * C), sc=(0, T * D), kob=C // 32)
+        for i, ((k, s), (w, b)) in enumerate(zip(geo, pk["convs"])):
+            To, Fo = Ts[i + 1], Fs[i + 1]
+            c = self._buf(f"c{i + 2}", (2, B, Fo, To, C))
+            ops.gemm(To, C, k * k * C, a, 0, 0, w, C * k * k * C, k * k * C, c, C, c_plane=B * Fo * To * C, split_out=True, bias=b,
+                     act=ACT_RELU, nbx=Fo, nby=B, sc=(To * C, Fo * To * C), a_mode=_A_MODE[(k, s)], conv=(Th, Fh, C))
+            if i + 1 < len(geo):
+                s = geo[i + 1][1]
+                Th, Fh = -(-To // s), -(-Fo // s)
+                a = self._buf(f"c{i + 2}p", (B, 2 * s * s, Fh, Th, C), zero=True)
+                ops.call("espb_phase_split_f32", ops.ptr(c), B * Fo * To * C, B, Fo, To, C, s, Th, Fh, ops.ptr(a))
+                _count()
+        T, Fl = Ts[-1], Fs[-1]
+        ops.gemm(T, D, Fl * C, c, B * Fl * T * C, C, pk["out_w"], D * Fl * C, Fl * C, x, D, bias=pk["out_b"], alpha=alpha, R=pe,
+                 ldr=0 if pe is None else D, nbx=1, nby=B, sa=(T * C, Fl * T * C), sc=(0, T * D), kob=C // 32)
 
     def _ffn(self, x, xn, norm, weights, act, alpha):
         """x += alpha * w_2(act(w_1(LN(x))))  (PositionwiseFeedForward behind its pre-LayerNorm)."""

@@ -43,6 +43,8 @@ _SIGS = {
     "espb_layernorm_f32": [P, L, I, P, P, F, P, P, L, P],
     "espb_split_tf32_f32": [P, L, P, L, P],
     "espb_conv1_relu_f32": [P, I, I, I, P, P, I, P, I, I, I, I, P],
+    "espb_conv1_relu_phase_f32": [P, I, I, I, P, P, I, P, I, I, I, I, I, P],
+    "espb_phase_split_f32": [P, L, I, I, I, I, I, I, I, P, P],
     "espb_qu_qv_f32": [P, L, L, I, P, P, P, P, L, P],
     "espb_v_transpose_f32": [P, L, I, I, I, I, P, P, L, I, P],
     "espb_relpos_softmax_f32": [P, P, I, I, I, I, I, P, F, P, L, P],

@@ -73,7 +73,7 @@ def gemm(M, N, K, A, a_plane, lda, B, b_plane, ldb, C, ldc, *, c_plane=0, split_
         al = [lda, ldb, a_plane, b_plane, sa[0], sa[1], sb[0], sb[1], a_off, b_off]
         if any(v % 4 for v in al):
             use_tc = 0
-        if a_mode == 1 and conv[2] % 32:
+        if a_mode and conv[2] % 32:
             use_tc = 0
         if a_mode == 0 and kob > 0 and K % (kob * 32):
             use_tc = 0

@@ -1,10 +1,10 @@
-"""TransformerEncoder (absolute positions, conv2d input layer, pre-LN, ReLU feed-forward) with the reference's constructor /
+"""TransformerEncoder (absolute positions, conv2d / conv2d2 / conv2d6 / conv2d8 input layer, pre-LN, ReLU feed-forward) with the reference's constructor /
 state_dict surface -- the encoder of the next scope row (SURVEY.md 8f-1, BASELINE configs[4]).  It composes the kernels of the
 Conformer path (conv1 / implicit-GEMM conv2 / wgmma 3xTF32 GEMMs / LayerNorm) plus a plain masked softmax; the subsampling, FFN and
 self-attention are the shared ones of layers.py.
 
 Reference: espnet2/asr/encoder/transformer_encoder.py:43-299, legacy/nets/pytorch_backend/transformer/encoder_layer.py:65-126,
-attention.py:77-151,262-265 (default branch), embedding.py:38-95 (PositionalEncoding), subsampling.py:397-474.
+attention.py:77-151,262-265 (default branch), embedding.py:38-95 (PositionalEncoding), subsampling.py:386-862.
 Parity: tests/test_gpu_zz_next.py (reference fixture layer by layer, ragged batch, whole Speech2Text) and tests/test_host_logic_emulated.py; self-attention
 is the fused wgmma kernel without the rel-pos term (csrc/attention.cu) at d_k = 64.
 """
@@ -14,7 +14,7 @@ from typing import List, Optional, Tuple
 import torch
 
 from . import ops
-from .layers import LN_EPS, EncoderBase, _FFN, _MHA, abs_pos_table
+from .layers import LN_EPS, SUBSAMPLING, EncoderBase, _FFN, _MHA, abs_pos_table
 # call / ptr / gemm stay importable here although the shared code in layers.py launches: the kernel emulation of the tests replaces
 # these names in every encoder module
 from .lib import call, ptr  # noqa: F401
@@ -39,13 +39,13 @@ class TransformerEncoder(EncoderBase):
                  normalize_before: bool = True, concat_after: bool = False, positionwise_layer_type: str = "linear",
                  positionwise_conv_kernel_size: int = 1, padding_idx: int = -1, interctc_layer_idx: List[int] = [],
                  interctc_use_conditioning: bool = False, layer_drop_rate: float = 0.0, qk_norm: bool = False, use_flash_attn: bool = True):
-        if (input_layer != "conv2d" or pos_enc_layer_type != "abs_pos" or not normalize_before or concat_after
+        if (input_layer not in SUBSAMPLING or pos_enc_layer_type != "abs_pos" or not normalize_before or concat_after
                 or positionwise_layer_type != "linear" or qk_norm or len(interctc_layer_idx)):
-            raise NotImplementedError("espnet_b200 TransformerEncoder: conv2d input, abs_pos, pre-LN, linear feed-forward, no interCTC / qk_norm")
+            raise NotImplementedError("espnet_b200 TransformerEncoder: conv2d / conv2d2 / conv2d6 / conv2d8 input, abs_pos, pre-LN, linear feed-forward, no interCTC / qk_norm")
         assert output_size % attention_heads == 0
         if output_size % 32:
             raise NotImplementedError("espnet_b200 TransformerEncoder: output_size must be a multiple of 32")
-        super().__init__(input_size, output_size, (_Layer(output_size, linear_units) for _ in range(num_blocks)))
+        super().__init__(input_size, output_size, (_Layer(output_size, linear_units) for _ in range(num_blocks)), input_layer)
         self.heads, self.num_blocks = attention_heads, num_blocks
         self._pe = {}
 

@@ -29,17 +29,22 @@ const char* espb_last_error(void);
 int espb_abi_version(void);
 int espb_device_sm(int* major, int* minor);
 
-/* ---- GEMM: every nn.Linear / 1x1 Conv1d / Conv2d(3x3,s2) / batched attention matmul on the path --------------
+/* ---- GEMM: every nn.Linear / 1x1 Conv1d / Conv2d(C,C,k,s) / batched attention matmul on the path --------------
  * C[by,bx] = R + alpha * act(A[by,bx] (M x K) * B[by,bx]^T (N x K) + bias), operands split (hi/lo planes).
  * Replaces torch.matmul / F.linear at: positionwise_feed_forward.py:30-32, attention.py:77-119,146,448-452,
- * convolution.py:66,77 (pointwise convs), subsampling.py:400-406,451 (conv2 as implicit GEMM a_mode=1, embed.out
+ * convolution.py:66,77 (pointwise convs), subsampling.py:400-406,451,606-611,711-716,818-825 (convs as implicit GEMM a_mode 1..3, embed.out
  * with kob), ctc.py:39 (ctc_lo), transformer_decoder.py:227-234 (output_layer), decoder_layer.py (all Linears).
  * use_tc=1: wgmma tf32, 3 MMAs per product (A_lo*B_hi + A_hi*B_lo + A_hi*B_hi), TMA operands
  *           (needs 16-byte aligned bases/strides); use_tc=0: SIMT fp32 FFMA kernel, any strides. */
 typedef struct EspbGemmDesc {
   int M, N, K;
   int nbx, nby;
-  int a_mode;          /* 0 general; 1 conv2 implicit GEMM over the parity-split conv1 output */
+  int a_mode;          /* 0 general; 1..3 implicit-GEMM Conv2d(C, C, k, s) over an input split into its s*s phases
+                          [b][plane*s*s + (t%s)*s + (f%s)][cv_f1h][cv_t1h][C] (espb_conv1_relu_phase_f32, espb_phase_split_f32):
+                          row m = output time, batch x = output frequency, K = k*k*C ordered (kt, kf, c), nby = batch;
+                          1: k 3, s 2 (subsampling.py:400-406 Conv2dSubsampling; Conv2dSubsampling8 :818-825, both strided convs);
+                          2: k 3, s 1 (Conv2dSubsampling2, subsampling.py:606-611);
+                          3: k 5, s 3 (Conv2dSubsampling6, subsampling.py:711-716) */
   int kob;             /* mode 0: K blocks (32) per outer A index; <=0 none */
   const float* A; long long a_plane, lda, sa_x, sa_y;
   const float* B; long long b_plane, ldb, sb_x, sb_y;
@@ -49,7 +54,7 @@ typedef struct EspbGemmDesc {
   const float* R; long long ldr, sr_x, sr_y;
   float alpha;
   int act;
-  int cv_t1h, cv_f1h, cv_cin;
+  int cv_t1h, cv_f1h, cv_cin;   /* a_mode 1..3: ceil(T_in/s), ceil(F_in/s) of the conv input, its channel count (a multiple of 32) */
   int band_t;          /* > 0: rel-pos band -- only elements of row m in columns [band_t-1-m, 2*band_t-2-m] are defined in C afterwards
                           (the band kernel serves a_mode 0, K <= 128 and the plain epilogue; other descriptors compute all of C) */
 } EspbGemmDesc;
@@ -81,9 +86,17 @@ int espb_layernorm_f32(const float* x, long long rows, int D, const float* gamma
                        float* out_split, long long split_plane, cudaStream_t stream);
 /* fp32 -> tf32 hi/lo planes (weights, positional table). */
 int espb_split_tf32_f32(const float* x, long long n, float* out, long long plane, cudaStream_t stream);
-/* Conv2d(1,C,3,2)+ReLU (subsampling.py:400-402): feats [B][Tf_max][F] -> [B][8][F1h][T1h][C] parity-split planes. */
+/* Conv2d(1,C,3,2)+ReLU (subsampling.py:400-402): feats [B][Tf_max][F] -> [B][8][F1h][T1h][C] parity-split planes
+ * (espb_conv1_relu_phase_f32 with s = 2). */
 int espb_conv1_relu_f32(const float* feats, int B, int Tf_max, int F, const float* w, const float* bias, int C, float* out, int T1, int F1,
                         int T1h, int F1h, cudaStream_t stream);
+/* The first Conv2d(1,C,3,2)+ReLU of Conv2dSubsampling2/6/8 (subsampling.py:606-611,711-716,818-825) with its output split into the s*s
+ * phases of the next conv's stride s in 1..3: [B][plane*s*s + (t1%s)*s + (f1%s)][F1h][T1h][C], F1h = ceil(F1/s), T1h = ceil(T1/s). */
+int espb_conv1_relu_phase_f32(const float* feats, int B, int Tf_max, int F, const float* w, const float* bias, int C, float* out, int T1, int F1,
+                              int s, int T1h, int F1h, cudaStream_t stream);
+/* Conv2dSubsampling8's second conv output -> input of its third (subsampling.py:818-825): x split [B][F][T][C] (planes x_plane apart) ->
+ * [B][plane*s*s + (t%s)*s + (f%s)][Fh][Th][C] with Fh = ceil(F/s), Th = ceil(T/s); C, x_plane multiples of 4, x / out 16-byte aligned. */
+int espb_phase_split_f32(const float* x, long long x_plane, int B, int F, int T, int C, int s, int Th, int Fh, float* out, cudaStream_t stream);
 /* q + pos_bias_u / q + pos_bias_v (attention.py:441-444) from the split qkv buffer [M][3D]. */
 int espb_qu_qv_f32(const float* qkv, long long qkv_plane, long long M, int D, const float* pos_u, const float* pos_v, float* qu, float* qv,
                    long long out_plane, cudaStream_t stream);
