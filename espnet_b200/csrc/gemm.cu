@@ -3,12 +3,13 @@
 // cannot address).
 //
 // The tensor-core kernel is persistent: min(tiles, SMs) CTAs, CTA c takes 128 x BN output tiles c, c + gridDim.x, ... (see tile_at for
-// the order).  Warp roles per CTA (288 threads):
-//   warps 0-7: two consumer warpgroups; warpgroup g issues the wgmma for rows [64g, 64g+64) of each tile and runs their epilogue
-//              (bias / activation / residual / hi-lo split) straight from the accumulator registers
-//   warp 8   : TMA producer (one elected lane) -> full[s]; the consumers release a stage through empty[s] once its MMAs retired.  The
-//              producer walks the CTA's tiles in the same order, so the next tile's first k-blocks load during the current tile's last
-//              MMAs and its epilogue.
+// the order).  Warp roles per CTA (512 threads):
+//   warps 0-7 : two consumer warpgroups; warpgroup g issues the wgmma for rows [64g, 64g+64) of each tile, writes the finished fp32
+//               accumulators into a shared-memory staging buffer and starts the next tile's MMAs at once
+//   warp 8    : TMA producer (one elected lane) -> full[s]; the consumers release a stage through empty[s] once its MMAs retired.  The
+//               producer walks the CTA's tiles in the same order, so the ring runs on across tile boundaries.
+//   warps 9-15: epilogue: read each staged 64 x BN half-tile, apply bias / activation / alpha / residual / hi-lo split and store it with
+//               row-contiguous 16-byte accesses, while the consumers run the next tile's MMAs.
 // The rel-pos band product (EspbGemmDesc::band_t > 0) has its own persistent kernel, relpos_band_kernel.
 #include <cuda.h>
 #include <limits.h>
@@ -29,7 +30,17 @@ using namespace espb::tc;
 constexpr int BM = 128;
 constexpr int BK = 32;                  // 32 fp32 = 128 B = one swizzle row
 constexpr int A_TILE_BYTES = BM * 128;  // one plane
-constexpr int NUM_THREADS = 288;
+constexpr int NUM_THREADS = 512;
+constexpr int EPI_WARP0 = 9;            // warps 9-15 run the epilogue
+constexpr int EPI_THREADS = NUM_THREADS - EPI_WARP0 * 32;
+constexpr int STAGING_BYTES = 32768;    // 64 x 128 fp32 (one warpgroup's 128-column half-tile, or both warpgroups' 64-column ones)
+// Registers per thread after setmaxnreg.  setmaxnreg only moves registers inside the CTA's allocation, 512 x 128 (the launch bound's
+// per-thread limit), so the two consumer and two producer / epilogue warpgroups may not ask for more than 4 x 128 between them: a larger
+// request never completes.  The consumers hold two 64 x BN fp32 accumulator sets; the epilogue loop needs far fewer.
+constexpr int LAUNCH_REGS = (65536 / NUM_THREADS) & ~7;
+constexpr int CONSUMER_REGS = 176;
+constexpr int EPI_REGS = 80;
+static_assert(2 * CONSUMER_REGS + 2 * EPI_REGS <= 4 * LAUNCH_REGS, "setmaxnreg split exceeds the CTA's registers");
 // Chunked promotion (version 2): K is walked in chunks of CHUNK_KB k-blocks that accumulate in a fresh wgmma accumulator, which is
 // then added into an fp32 register accumulator with round-to-nearest, so the long accumulation chain does not run in the tensor core.
 constexpr int CHUNK_KB = 4;
@@ -75,20 +86,20 @@ __device__ __forceinline__ TilePos tile_at(const EspbGemmDesc& p, long long t, i
   return tp;
 }
 
-// Pair (col, col + 1) of a row of a bias or residual operand; columns past N read as 0.
-__device__ __forceinline__ float2 ld_pair(const float* ptr, int col, int N, bool vec) {
-  if (col + 1 < N) {
-    if (vec) return *reinterpret_cast<const float2*>(ptr + col);
-    return make_float2(ptr[col], ptr[col + 1]);
-  }
-  return make_float2(col < N ? ptr[col] : 0.f, 0.f);
+// Four columns col..col + 3 of a row of a bias or residual operand; columns past N read as 0.  vec: ptr + col is 16-byte aligned.
+__device__ __forceinline__ float4 ld_quad(const float* ptr, int col, int N, bool vec) {
+  if (vec && col + 3 < N) return *reinterpret_cast<const float4*>(ptr + col);
+  float v[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) v[i] = col + i < N ? ptr[col + i] : 0.f;
+  return make_float4(v[0], v[1], v[2], v[3]);
 }
-__device__ __forceinline__ float2 ldg_pair(const float* ptr, int col, int N, bool vec) {
-  if (col + 1 < N) {
-    if (vec) return __ldg(reinterpret_cast<const float2*>(ptr + col));
-    return make_float2(__ldg(ptr + col), __ldg(ptr + col + 1));
-  }
-  return make_float2(col < N ? __ldg(ptr + col) : 0.f, 0.f);
+__device__ __forceinline__ float4 ldg_quad(const float* ptr, int col, int N, bool vec) {
+  if (vec && col + 3 < N) return __ldg(reinterpret_cast<const float4*>(ptr + col));
+  float v[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) v[i] = col + i < N ? __ldg(ptr + col + i) : 0.f;
+  return make_float4(v[0], v[1], v[2], v[3]);
 }
 
 // epi_value with the bias and residual values already loaded.
@@ -101,67 +112,104 @@ __device__ __forceinline__ float epi_apply(const EpiArgs& e, float acc, float b,
   return v;
 }
 
-// Stores two horizontally adjacent epilogue values (row, col) and (row, col + 1).
-__device__ __forceinline__ void epi_store2(const EpiArgs& e, int row, int col, float t0, float t1, int M, int N, bool vec_ok) {
-  if (row >= M || col >= N) return;
+// Stores four horizontally adjacent epilogue values (row, col..col + 3).  vec: 16-byte stores are aligned (ldc, c_plane, the slice
+// offset and C itself); otherwise, and at the last columns of a ragged N, element by element.
+__device__ __forceinline__ void epi_store4(const EpiArgs& e, int row, int col, const float (&t)[4], int N, bool vec) {
   float* crow = e.C + (long long)row * e.ldc;
-  const bool two = col + 1 < N;
-  if (vec_ok && two) {
+  if (vec && col + 3 < N) {
     if (e.split_out) {
-      const float h0 = espb::tf32_hi(t0), h1 = espb::tf32_hi(t1);
-      *reinterpret_cast<float2*>(crow + col) = make_float2(h0, h1);
-      *reinterpret_cast<float2*>(crow + e.c_plane + col) = make_float2(espb::tf32_lo(t0, h0), espb::tf32_lo(t1, h1));
+      float h[4], l[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) { h[i] = espb::tf32_hi(t[i]); l[i] = espb::tf32_lo(t[i], h[i]); }
+      *reinterpret_cast<float4*>(crow + col) = make_float4(h[0], h[1], h[2], h[3]);
+      *reinterpret_cast<float4*>(crow + e.c_plane + col) = make_float4(l[0], l[1], l[2], l[3]);
     } else {
-      *reinterpret_cast<float2*>(crow + col) = make_float2(t0, t1);
+      *reinterpret_cast<float4*>(crow + col) = make_float4(t[0], t[1], t[2], t[3]);
     }
     return;
   }
-  const float t[2] = {t0, t1};
-  for (int i = 0; i < (two ? 2 : 1); ++i) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    if (col + i >= N) break;
     if (e.split_out) { const float h = espb::tf32_hi(t[i]); crow[col + i] = h; crow[e.c_plane + col + i] = espb::tf32_lo(t[i], h); }
     else crow[col + i] = t[i];
   }
 }
 
-// Epilogue of one warpgroup's 64 x BN accumulator tile, in groups of EPI_J 8-column slices.  Each group issues all its bias and residual
-// loads before its first store, so the loads of a group overlap: R is either C itself (each element read and then written by the same
-// thread) or disjoint from C (gemm.h), so no store can feed a load.  With EPI_J = 4 the loaded values, the accumulators and what lives
-// across the out-of-line GELU call fit the 168 registers ptxas gives a thread of this 288-thread CTA; EPI_J = 8 spills.
-constexpr int EPI_J = 4;
+// Staging buffer of one 64 x BN half-tile: row r at r * BN floats, its 16-byte chunk q at chunk q ^ 2 (r & 3).  The consumers' 8-byte
+// fragment stores (a half-warp writes two chunks of each of 4 consecutive rows) and the epilogue's row-contiguous 16-byte loads are
+// then both free of bank conflicts.
+template <int BN>
+__device__ __forceinline__ uint32_t staging_off(int r, int c) {
+  return (uint32_t)(r * BN + ((((c >> 2) ^ ((r & 3) << 1))) << 2) + (c & 3)) * 4u;
+}
+
+// One warpgroup's finished 64 x BN accumulators (fragment layout, tc_common.cuh) into the staging buffer at buf.
+template <int BN>
+__device__ __forceinline__ void stage_tile(uint32_t buf, const float (&d)[BN / 2], int r0, int c0) {
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(buf + staging_off<BN>(r0 + 8 * h, c0 + 8 * j)), "f"(d[4 * j + 2 * h]),
+                   "f"(d[4 * j + 2 * h + 1])
+                   : "memory");
+}
+
+__device__ __forceinline__ float4 ld_shared_f4(uint32_t addr) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
+  return v;
+}
+
+// Epilogue warps: every tile of this CTA, its two 64-row halves in order.  A thread owns four columns of the tile (the bias values are
+// loaded once per tile) and a row every RPP rows; the residual loads of EPI_U such rows are issued before the first of them is stored.  R is
+// either C itself (each element read and then written by the same thread) or disjoint from C (gemm.h), so no store can feed a load.
+constexpr int EPI_U = 4;
 
 template <int BN>
-__device__ __forceinline__ void epilogue(const EspbGemmDesc& p, const TilePos& tp, const float (&d)[BN / 2], int row, int col) {
-  constexpr int G = BN / 8 < EPI_J ? BN / 8 : EPI_J;
-  EpiArgs e;
-  const long long coff = (long long)tp.by * p.sc_y + (long long)tp.bx * p.sc_x;
-  const long long roff = (long long)tp.by * p.sr_y + (long long)tp.bx * p.sr_x;
-  e.C = p.C + coff; e.c_plane = p.c_plane; e.ldc = p.ldc; e.split_out = p.split_out;
-  e.bias = p.bias ? p.bias + (long long)tp.bx * p.sbias_x : nullptr; e.R = p.R ? p.R + roff : nullptr;
-  e.ldr = p.ldr; e.alpha = p.alpha; e.act = p.act;
-  const bool vec_ok = ((p.ldc & 1) == 0) && ((coff & 1) == 0) && ((p.c_plane & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 7) == 0);
-  const bool bias_vec = (reinterpret_cast<uintptr_t>(e.bias) & 7) == 0;
-  const bool r_vec = ((p.ldr & 1) == 0) && ((reinterpret_cast<uintptr_t>(e.R) & 7) == 0);
+__device__ __forceinline__ void epilogue_warps(const EspbGemmDesc& p, long long ntiles, int tiles_m, int tiles_n, int band, uint32_t staging,
+                                               uint32_t stg_full, uint32_t stg_empty) {
+  constexpr int NBUF = STAGING_BYTES / (64 * BN * 4);   // 1: the warpgroups take turns on one buffer; 2: one buffer each
+  constexpr int TPR = BN / 4, RPP = EPI_THREADS / TPR;  // threads per row, rows per pass
+  const int et = threadIdx.x - EPI_WARP0 * 32;
+  const int r_first = et / TPR, cc = 4 * (et % TPR);
+  int it = 0;   // this CTA's tile ordinal: selects the staging barriers' phase
+  for (long long t = blockIdx.x; t < ntiles; t += gridDim.x, ++it) {
+    const TilePos tp = tile_at<BN>(p, t, tiles_m, tiles_n, band);
+    EpiArgs e;
+    const long long coff = (long long)tp.by * p.sc_y + (long long)tp.bx * p.sc_x;
+    const long long roff = (long long)tp.by * p.sr_y + (long long)tp.bx * p.sr_x;
+    e.C = p.C + coff; e.c_plane = p.c_plane; e.ldc = p.ldc; e.split_out = p.split_out;
+    e.bias = p.bias ? p.bias + (long long)tp.bx * p.sbias_x : nullptr; e.R = p.R ? p.R + roff : nullptr;
+    e.ldr = p.ldr; e.alpha = p.alpha; e.act = p.act;
+    const bool c_vec = ((p.ldc & 3) == 0) && ((coff & 3) == 0) && ((p.c_plane & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
+    const bool r_vec = ((p.ldr & 3) == 0) && ((reinterpret_cast<uintptr_t>(e.R) & 15) == 0);
+    const int col = tp.n0 + cc;
+    const float4 bv = e.bias ? ldg_quad(e.bias, col, p.N, (reinterpret_cast<uintptr_t>(e.bias) & 15) == 0) : make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int g = 0; g < 2; ++g) {
+      mbar_wait(stg_full + 8 * g, (uint32_t)it & 1);
+      const uint32_t buf = staging + (NBUF == 1 ? 0 : g) * (64 * BN * 4);
+      const int row_base = tp.m0 + 64 * g;
+#pragma unroll 1
+      for (int r0 = r_first; r0 < 64; r0 += EPI_U * RPP) {
+        float4 rv[EPI_U];
 #pragma unroll
-  for (int j0 = 0; j0 < BN / 8; j0 += G) {
-    float2 bv[G], rv[G][2];
+        for (int u = 0; u < EPI_U; ++u) {
+          const int r = r0 + u * RPP, row = row_base + r;
+          rv[u] = (e.R && r < 64 && row < p.M) ? ld_quad(e.R + (long long)row * e.ldr, col, p.N, r_vec) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
 #pragma unroll
-    for (int j = 0; j < G; ++j) {
-      const int c = col + 8 * (j0 + j);
-      bv[j] = e.bias ? ldg_pair(e.bias, c, p.N, bias_vec) : make_float2(0.f, 0.f);
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int r = row + 8 * h;
-        rv[j][h] = (e.R && r < p.M) ? ld_pair(e.R + (long long)r * e.ldr, c, p.N, r_vec) : make_float2(0.f, 0.f);
+        for (int u = 0; u < EPI_U; ++u) {
+          const int r = r0 + u * RPP, row = row_base + r;
+          if (r >= 64 || row >= p.M) break;
+          const float4 a = ld_shared_f4(buf + staging_off<BN>(r, cc));
+          const float v[4] = {epi_apply(e, a.x, bv.x, rv[u].x), epi_apply(e, a.y, bv.y, rv[u].y), epi_apply(e, a.z, bv.z, rv[u].z),
+                              epi_apply(e, a.w, bv.w, rv[u].w)};
+          epi_store4(e, row, col, v, p.N, c_vec);
+        }
       }
-    }
-#pragma unroll
-    for (int j = 0; j < G; ++j) {
-      const int i = 4 * (j0 + j);
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const float t0 = epi_apply(e, d[i + 2 * h], bv[j].x, rv[j][h].x), t1 = epi_apply(e, d[i + 2 * h + 1], bv[j].y, rv[j][h].y);
-        epi_store2(e, row + 8 * h, col + 8 * (j0 + j), t0, t1, p.M, p.N, vec_ok);
-      }
+      mbar_arrive_local(stg_empty + 8 * (NBUF == 1 ? g ^ 1 : g));   // with one buffer, half g's release lets the other warpgroup write
     }
   }
 }
@@ -173,9 +221,12 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   constexpr int B_TILE_BYTES = BN * 128;
   constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
   constexpr int NR = BN / 2;   // accumulator registers per thread: a 64 x BN warpgroup tile over 128 threads
+  constexpr int NBUF = STAGING_BYTES / (64 * BN * 4);
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t full_bar = smem_base + STAGES * STAGE_BYTES, empty_bar = full_bar + 8 * STAGES;
+  const uint32_t staging = smem_base + STAGES * STAGE_BYTES;
+  const uint32_t full_bar = staging + STAGING_BYTES, empty_bar = full_bar + 8 * STAGES;
+  const uint32_t stg_full = empty_bar + 8 * STAGES, stg_empty = stg_full + 16;   // per consumer warpgroup
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_kb = (p.K + BK - 1) / BK;
@@ -183,6 +234,7 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 2); }   // empty: one arrival per consumer warpgroup
+    for (int g = 0; g < 2; ++g) { mbar_init(stg_full + 8 * g, 128); mbar_init(stg_empty + 8 * g, EPI_THREADS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
@@ -191,7 +243,12 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   espb::pdl_trigger();   // barriers and descriptors are ready: the next kernel may start its own setup
   espb::pdl_wait();      // first global access (TMA loads of A / B) follows
 
-  if (warp == 8) {
+  if (warp >= 8) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(EPI_REGS));
+    if (warp >= EPI_WARP0) {
+      epilogue_warps<BN>(p, ntiles, tiles_m, tiles_n, band, staging, stg_full, stg_empty);
+      return;
+    }
     if (elect_one_sync()) {   // one lane, known to ptxas: uniform-datapath issue without per-instruction waterfall loops
       const int cblk = (p.a_mode != 0) ? p.cv_cin / BK : 0;
       const ConvGeom g = conv_geom(p.a_mode);
@@ -225,15 +282,19 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     return;
   }
 
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONSUMER_REGS));
   const int wg = warp >> 2;
   const bool wg_leader = (threadIdx.x & 127) == 0;
-  const int row_in_tile = wg * 64 + (warp & 3) * 16 + (lane >> 2), col_in_tile = 2 * (lane & 3);
+  const int row_in_half = (warp & 3) * 16 + (lane >> 2), col_in_tile = 2 * (lane & 3);
+  const uint32_t my_buf = staging + (NBUF == 1 ? 0 : wg) * (64 * BN * 4);
+  // With one staging buffer warpgroup 1 writes after the epilogue read warpgroup 0's half of the same tile: its first wait blocks.
+  const uint32_t stg_parity0 = (NBUF == 1 && wg == 1) ? 0u : 1u;
   int s = 0;
   uint32_t ph = 0;
   float acc[NR], part[NR];
-  for (long long t = blockIdx.x; t < ntiles; t += gridDim.x) {
-    const TilePos tp = tile_at<BN>(p, t, tiles_m, tiles_n, band);
-    // part is overwritten by the first MMA (scale-d 0); zeroing it here keeps it dead, not live in registers, across the epilogue
+  int it = 0;   // this CTA's tile ordinal
+  for (long long t = blockIdx.x; t < ntiles; t += gridDim.x, ++it) {
+    // part is overwritten by the first MMA (scale-d 0); zeroing it here keeps it dead, not live in registers, across the handoff
 #pragma unroll
     for (int i = 0; i < NR; ++i) { acc[i] = 0.f; part[i] = 0.f; }
     // Each k-block's MMAs retire before its stage is released.  Keeping one k-block in flight (wait_group 1) would hold a second stage
@@ -264,7 +325,10 @@ gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       }
       if (++s == STAGES) { s = 0; ph ^= 1; }
     }
-    epilogue<BN>(p, tp, PROMOTE ? acc : part, tp.m0 + row_in_tile, tp.n0 + col_in_tile);
+    // hand the tile to the epilogue warps and go on with the next one
+    mbar_wait(stg_empty + 8 * wg, ((uint32_t)it & 1) ^ stg_parity0);
+    stage_tile<BN>(my_buf, PROMOTE ? acc : part, row_in_half, col_in_tile);
+    mbar_arrive_local(stg_full + 8 * wg);
   }
 }
 
@@ -588,7 +652,7 @@ int column_band(const EspbGemmDesc& d, int bn, int tiles_m, int tiles_n) {
 
 template <int BN, int STAGES, bool PROMOTE>
 int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const EspbGemmDesc& d, int bxm, int bym, int axm, int aym, cudaStream_t stream) {
-  constexpr int smem = STAGES * (2 * A_TILE_BYTES + 2 * BN * 128) + 1024 + 16 * STAGES;
+  constexpr int smem = STAGES * (2 * A_TILE_BYTES + 2 * BN * 128) + STAGING_BYTES + 1024 + 16 * STAGES + 32;
   static_assert(smem <= 232448, "dynamic shared memory budget exceeded");
   static bool attr_set = false;
   if (!attr_set) {
