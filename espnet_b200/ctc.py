@@ -2,26 +2,21 @@
 import torch
 
 from . import ops
+from .layers import PackedModule
 from .lib import call, ptr
 from .ops import _count, linear, split_from
 
 
-class CTC(torch.nn.Module):
+class CTC(PackedModule):
     def __init__(self, odim: int, encoder_output_size: int, dropout_rate: float = 0.0, ctc_type: str = "builtin",
                  reduce: bool = True, ignore_nan_grad=None, zero_infinity: bool = True, brctc_risk_strategy: str = "exp",
                  brctc_group_strategy: str = "end", brctc_risk_factor: float = 0.0):
         super().__init__()
         self.ctc_lo = torch.nn.Linear(encoder_output_size, odim)
         self.odim, self.eprojs = odim, encoder_output_size
-        self._packed = None
-
-    def _load_from_state_dict(self, *args, **kwargs):
-        self._packed = None
-        return super()._load_from_state_dict(*args, **kwargs)
 
     def _pack(self):
-        w = self.ctc_lo.weight.detach().float().contiguous()
-        self._packed = (split_from(w), self.ctc_lo.bias.detach().float().contiguous())
+        self._packed = (split_from(self._f32(self.ctc_lo.weight)), self._f32(self.ctc_lo.bias))
         return self._packed
 
     def _split_input(self, hs_pad, hs_split):

@@ -1,8 +1,9 @@
-"""Host code the four CUDA-path encoders share: the parameter containers (the reference's attribute names, created in the reference's order so
-that a seeded default init gives the same weights), the sinusoid tables, and ``EncoderBase`` -- the state every encoder has (packed weights,
-workspace, ``after_norm``) and the packing and launches of the blocks they have in common: Conv2dSubsampling, the feed-forward module, the
-convolution module, rel-pos and plain self-attention.  Each encoder module keeps its constructor checks, its layer container, the packing of
-its own weights and its per-layer sequence in ``forward``.
+"""Host code the CUDA-path modules share: the parameter containers (the reference's attribute names, created in the reference's order so
+that a seeded default init gives the same weights), the sinusoid tables, ``PackedModule`` -- the packed weights and workspace of every
+encoder, decoder, LM and CTC head, the packing of LayerNorm, attention and feed-forward weights and the feed-forward launches -- and
+``EncoderBase``, the state every encoder has (``after_norm``) and the packing and launches of the blocks they have in common:
+Conv2dSubsampling, the convolution module, rel-pos and plain self-attention.  Each encoder module keeps its constructor checks, its layer
+container, the packing of its own weights and its per-layer sequence in ``forward``.
 
 The torch.nn layers are parameter containers only (reference checkpoints load by name); forward never calls them.
 """
@@ -134,44 +135,42 @@ def _pitch(n):
     return (n + 31) // 32 * 32
 
 
-class EncoderBase(torch.nn.Module):
-    """``embed`` (Conv2dSubsampling), ``encoders`` (the layers, built from ``layers``) and ``after_norm``, created in this order as in the
-    reference, plus the packed weights and the workspace.  Subclasses set ``heads`` and ``num_blocks`` (and ``kernel`` with the convolution
-    module) and define ``_pack`` and ``forward``."""
+class PackedModule(torch.nn.Module):
+    """A module whose forward runs the kernels on device-side copies of its weights (``_packed``, built by the subclass's ``_pack`` and
+    dropped when a state_dict loads) and on a workspace of named buffers kept across calls (``_buf``)."""
 
-    trace = None            # set to a list to collect per-stage outputs (tests)
-    last_split_out = None   # split copy of the last output (feeds the CTC head / decoder memory GEMMs)
+    ws_tag = 0          # workspace set in use: the search runs independent utterance groups on separate streams, each with its own buffers
+    zero_bufs = False   # True: every workspace buffer is zero-filled when (re)created, not only those asked for with zero=True
 
-    def __init__(self, input_size, output_size, layers, input_layer="conv2d"):
+    def __init__(self):
         super().__init__()
-        self._output_size, self.idim, self.input_layer = output_size, input_size, input_layer
-        self.embed = _Conv2dSubsampling(input_size, output_size, input_layer)
-        self.encoders = torch.nn.ModuleList(layers)
-        self.after_norm = torch.nn.LayerNorm(output_size, eps=LN_EPS)
         self._packed, self._ws = None, {}
-        self._pos_cache = {}   # rel-pos encoders: _pos per length
-
-    def output_size(self) -> int:
-        return self._output_size
+        self.buf_version = 0   # bumped on every allocation: captured CUDA graphs hold the buffers' pointers
 
     def _load_from_state_dict(self, *args, **kwargs):
         self._packed = None
         return super()._load_from_state_dict(*args, **kwargs)
 
+    @property
+    def _device(self):
+        return next(self.parameters()).device
+
     def _buf(self, name, shape, zero=False, dtype=torch.float32):
         """Workspace tensor kept across calls; a new shape or dtype replaces the buffer of that name (freed before the allocation)."""
+        name = (self.ws_tag, name)
         key = (name, tuple(shape), dtype)
         t = self._ws.get(key)
         if t is None:
             for k in [k for k in self._ws if k[0] == name]:
                 del self._ws[k]
-            t = (torch.zeros if zero else torch.empty)(shape, dtype=dtype, device=self.after_norm.weight.device)
+            t = (torch.zeros if zero or self.zero_bufs else torch.empty)(shape, dtype=dtype, device=self._device)
             self._ws[key] = t
+            self.buf_version += 1
         return t
 
     # ---------------------------------------------------------------- weights -> device-side packed/split form
     def _f32(self, t):
-        return t.detach().to(device=self.after_norm.weight.device, dtype=torch.float32).contiguous()
+        return t.detach().to(device=self._device, dtype=torch.float32).contiguous()
 
     def _pack_ln(self, m):
         return self._f32(m.weight), self._f32(m.bias)
@@ -189,6 +188,35 @@ class EncoderBase(torch.nn.Module):
         if isinstance(a, _PosBias):
             d["pos_u"], d["pos_v"] = f32(a.pos_bias_u).view(-1), f32(a.pos_bias_v).view(-1)
         return d
+
+    # ---------------------------------------------------------------- launches
+    def _ffn(self, x, xn, norm, weights, act, alpha=1.0):
+        """x += alpha * w_2(act(w_1(LN(x))))  (PositionwiseFeedForward behind its pre-LayerNorm)."""
+        w1, b1, w2, b2 = weights
+        h = self._buf("h", (2, x.shape[0], w1.shape[1]))
+        layernorm(x, *norm, LN_EPS, out_split=xn)
+        linear(xn, w1, h, bias=b1, act=act, split_out=True)
+        linear(h, w2, x, bias=b2, residual=x, alpha=alpha)
+
+
+class EncoderBase(PackedModule):
+    """``embed`` (Conv2dSubsampling), ``encoders`` (the layers, built from ``layers``) and ``after_norm``, created in this order as in the
+    reference.  Subclasses set ``heads`` and ``num_blocks`` (and ``kernel`` with the convolution module) and define ``_pack`` and
+    ``forward``."""
+
+    trace = None            # set to a list to collect per-stage outputs (tests)
+    last_split_out = None   # split copy of the last output (feeds the CTC head / decoder memory GEMMs)
+
+    def __init__(self, input_size, output_size, layers, input_layer="conv2d"):
+        super().__init__()
+        self._output_size, self.idim, self.input_layer = output_size, input_size, input_layer
+        self.embed = _Conv2dSubsampling(input_size, output_size, input_layer)
+        self.encoders = torch.nn.ModuleList(layers)
+        self.after_norm = torch.nn.LayerNorm(output_size, eps=LN_EPS)
+        self._pos_cache = {}   # rel-pos encoders: _pos per length
+
+    def output_size(self) -> int:
+        return self._output_size
 
     def _pack_pos(self, attns):
         """linear_pos of every attention layer stacked [L*D][D], L = the number of attention layers (layer ordinal a at rows a*D..): one GEMM
@@ -283,14 +311,6 @@ class EncoderBase(torch.nn.Module):
         ops.gemm(T, D, Fl * C, c, B * Fl * T * C, C, pk["out_w"], D * Fl * C, Fl * C, x, D, bias=pk["out_b"], alpha=alpha, R=pe,
                  ldr=0 if pe is None else D, nbx=1, nby=B, sa=(T * C, Fl * T * C), sc=(0, T * D), kob=C // 32)
 
-    def _ffn(self, x, xn, norm, weights, act, alpha):
-        """x += alpha * w_2(act(w_1(LN(x))))  (PositionwiseFeedForward behind its pre-LayerNorm)."""
-        w1, b1, w2, b2 = weights
-        h = self._buf("h", (2, x.shape[0], w1.shape[1]))
-        layernorm(x, *norm, LN_EPS, out_split=xn)
-        linear(xn, w1, h, bias=b1, act=act, split_out=True)
-        linear(h, w2, x, bias=b2, residual=x, alpha=alpha)
-
     def _conv_module(self, x, xn, norm, w, nseq, S, lens):
         """x += ConvolutionModule(LN(x))  (convolution.py:56-79) over nseq sequences of S rows; sequence b sees zeros outside rows
         0..lens[b]-1.  GLU, depthwise conv, BatchNorm and swish run as one kernel between the two pointwise GEMMs."""
@@ -327,7 +347,7 @@ class EncoderBase(torch.nn.Module):
             if len(self._pos_cache) > 8:
                 self._pos_cache.clear()
             D, LD = self._output_size, self._packed["pos_w_all"].shape[1]
-            pe = split_from(rel_pos_table(T, D).to(self.after_norm.weight.device))
+            pe = split_from(rel_pos_table(T, D).to(self._device))
             out = ops.new_split(2 * T - 1, LD, device=pe.device)
             linear(pe, self._packed["pos_w_all"], out, split_out=True)
             self._pos_cache[T] = out

@@ -17,9 +17,11 @@ from typing import Any, List, Tuple
 
 import torch
 
-from .layers import LN_EPS, _FFN, _MHA, abs_pos_table
+from . import ops
+from .decoder import KVCacheScorer, ScorerProtocol
+from .layers import LN_EPS, _FFN, _MHA, PackedModule
 from .lib import call, ptr
-from .ops import ACT_RELU, _count, layernorm, linear, new_split, split_from
+from .ops import ACT_RELU, _count, layernorm, linear, split_from
 
 
 class _LMLayer(torch.nn.Module):
@@ -40,7 +42,7 @@ class _LMEncoder(torch.nn.Module):
         self.after_norm = torch.nn.LayerNorm(d, eps=LN_EPS)
 
 
-class TransformerLM(torch.nn.Module):
+class TransformerLM(KVCacheScorer):
     """Drop-in container for espnet2.lm.transformer_lm.TransformerLM (inference scorer)."""
 
     def __init__(self, vocab_size: int, pos_enc: str = None, embed_unit: int = 128, att_unit: int = 256, head: int = 2, unit: int = 1024,
@@ -55,45 +57,24 @@ class TransformerLM(torch.nn.Module):
         self.embed = torch.nn.Embedding(vocab_size, embed_unit)
         self.encoder = _LMEncoder(embed_unit, att_unit, unit, layer)
         self.decoder = torch.nn.Linear(att_unit, vocab_size)
-        self._packed = None
-        self._ws = {}
-
-    def _load_from_state_dict(self, *args, **kwargs):
-        self._packed = None
-        return super()._load_from_state_dict(*args, **kwargs)
 
     def _pack(self):
-        dev = self.decoder.weight.device
-        f32 = lambda t: t.detach().to(device=dev, dtype=torch.float32).contiguous()  # noqa: E731
-        e = self.encoder
+        f32, e = self._f32, self.encoder
         pk = dict(emb=f32(self.embed.weight), in_w=split_from(f32(e.embed[0].weight)), in_b=f32(e.embed[0].bias),
-                  in_ln=(f32(e.embed[1].weight), f32(e.embed[1].bias), float(e.embed[1].eps)), layers=[])
+                  in_ln=(*self._pack_ln(e.embed[1]), float(e.embed[1].eps)), layers=[])
         for lyr in e.encoders:
-            sa, ff = lyr.self_attn, lyr.feed_forward
-            pk["layers"].append(dict(
-                n1=(f32(lyr.norm1.weight), f32(lyr.norm1.bias)), n2=(f32(lyr.norm2.weight), f32(lyr.norm2.bias)),
-                qkv_w=split_from(torch.cat([f32(sa.linear_q.weight), f32(sa.linear_k.weight), f32(sa.linear_v.weight)], 0)),
-                qkv_b=torch.cat([f32(sa.linear_q.bias), f32(sa.linear_k.bias), f32(sa.linear_v.bias)], 0),
-                so_w=split_from(f32(sa.linear_out.weight)), so_b=f32(sa.linear_out.bias),
-                w1=split_from(f32(ff.w_1.weight)), b1=f32(ff.w_1.bias), w2=split_from(f32(ff.w_2.weight)), b2=f32(ff.w_2.bias)))
-        pk["an"] = (f32(e.after_norm.weight), f32(e.after_norm.bias))
+            pk["layers"].append(dict(**self._pack_mha(lyr.self_attn), n1=self._pack_ln(lyr.norm1), n2=self._pack_ln(lyr.norm2),
+                                     ffn=self._pack_ffn(lyr.feed_forward)))
+        pk["an"] = self._pack_ln(e.after_norm)
         pk["out_w"], pk["out_b"] = split_from(f32(self.decoder.weight)), f32(self.decoder.bias)
         self._packed = pk
         return pk
 
-    ws_tag = 0
-
-    def _buf(self, name, shape, dtype=torch.float32):
-        name = (self.ws_tag, name)
-        key = (name, tuple(shape), dtype)
-        t = self._ws.get(key)
-        if t is None:
-            for k in [k for k in self._ws if k[0] == name]:
-                del self._ws[k]
-            t = torch.empty(shape, dtype=dtype, device=self.decoder.weight.device)
-            self._ws[key] = t
-            self.buf_version = getattr(self, "buf_version", 0) + 1   # captured CUDA graphs hold these pointers
-        return t
+    def _iface_state(self, xs, n, need_len):
+        st = getattr(self, "_iface_st", None)
+        if st is None or st["n"] != n or st["max_len"] < need_len:
+            st = self._iface_st = self.init_cache(n, max(32, 1 << (need_len - 1).bit_length()))
+        return st
 
     # ---------------------------------------------------------------- device-side incremental scorer
     @torch.no_grad()
@@ -101,12 +82,7 @@ class TransformerLM(torch.nn.Module):
         if self._packed is None:
             self._pack()
         L, D = self.num_blocks, self.d
-        pe = None
-        if self.pos_enc == "sinusoidal":
-            key = ("pe", max_len)
-            if key not in self._ws:
-                self._ws[key] = abs_pos_table(max_len, D).to(self.decoder.weight.device)
-            pe = self._ws[key]
+        pe = self._pe(max_len) if self.pos_enc == "sinusoidal" else None
         return dict(n=n_slots, max_len=max_len, kc=self._buf("kc", (L, max_len, n_slots, D)), vc=self._buf("vc", (L, max_len, n_slots, D)), pe=pe)
 
     @torch.no_grad()
@@ -114,13 +90,11 @@ class TransformerLM(torch.nn.Module):
         """One position for all n slots: log-probabilities [n][V] of the next token (buffer reused across steps).  Equivalent of
         batch_score (transformer_lm.py:95-133) for prefixes whose newest token is ``last_tok`` at position ``pos`` (+ *step_ptr)."""
         pk = self._packed
-        n, D, H, E, U = st["n"], self.d, self.heads, self.embed_unit, self.units
+        n, D, E = st["n"], self.d, self.embed_unit
         es = self._buf("es", (2, n, E))
         x = self._buf("x", (n, D))
         xn = self._buf("xn", (2, n, D))
-        qkv = self._buf("qkv", (n, 3 * D))
         ctx = self._buf("ctx", (2, n, D))
-        h = self._buf("h", (2, n, U))
         call("espb_gather_rows_split_f32", ptr(last_tok), ptr(pk["emb"]), n, E, ptr(es), n * E)
         _count()
         linear(es, pk["in_w"], x, bias=pk["in_b"])
@@ -128,51 +102,9 @@ class TransformerLM(torch.nn.Module):
         call("espb_relu_posenc_f32", ptr(x), n, D, ptr(st["pe"]), pos, ptr(step_ptr), math.sqrt(D))
         _count()
         for li, w in enumerate(pk["layers"]):
-            layernorm(x, *w["n1"], LN_EPS, out_split=xn)
-            linear(xn, w["qkv_w"], qkv, bias=w["qkv_b"])
-            call("espb_dec_self_attn_f32", ptr(qkv), ptr(st["kc"][li]), ptr(st["vc"][li]), ptr(anc), anc.shape[1], n, D, H, pos,
-                 ptr(step_ptr), st["max_len"], ptr(ctx), n * D)
-            _count()
-            linear(ctx, w["so_w"], x, bias=w["so_b"], residual=x)
-            layernorm(x, *w["n2"], LN_EPS, out_split=xn)
-            linear(xn, w["w1"], h, bias=w["b1"], act=ACT_RELU, split_out=True)
-            linear(h, w["w2"], x, bias=w["b2"], residual=x)
-        layernorm(x, *pk["an"], LN_EPS, out_split=xn)
-        logp = self._buf("logp", (n, self.vocab_size))
-        linear(xn, pk["out_w"], logp, bias=pk["out_b"])
-        from . import ops
-
-        ops.log_softmax_rows_(logp)
-        return logp
-
-    # ---------------------------------------------------------------- BatchScorerInterface (scorer_interface.py:85-188), as decoder.py
-    def init_state(self, x: torch.Tensor):
-        return None
-
-    def batch_init_state(self, x: torch.Tensor):
-        return None
-
-    def select_state(self, state, i: int, new_id: int = None):
-        return None if state is None else state[i]
-
-    def final_score(self, state) -> float:
-        return 0.0
-
-    @torch.no_grad()
-    def batch_score(self, ys: torch.Tensor, states: List[Any], xs: torch.Tensor) -> Tuple[torch.Tensor, List[Any]]:
-        n, ln = ys.shape
-        pos = ln - 1
-        self.ws_tag = "iface"
-        st = getattr(self, "_iface_st", None)
-        if st is None or st["n"] != n or st["max_len"] < ln:
-            st = self._iface_st = self.init_cache(n, max(32, 1 << (ln - 1).bit_length()))
-        if pos > 0:
-            st["kc"][:, :pos] = torch.stack([s[0] for s in states], dim=2)
-            st["vc"][:, :pos] = torch.stack([s[1] for s in states], dim=2)
-        anc = self._buf("iface_anc", (n, st["max_len"] + 1), dtype=torch.int32)
-        anc.copy_(torch.arange(n, dtype=torch.int32, device=anc.device).view(n, 1).expand_as(anc))
-        logp = self.step(st, pos, ys[:, -1].to(torch.int32).contiguous(), anc, None)
-        return logp.clone(), [(st["kc"][:, :ln, b].clone(), st["vc"][:, :ln, b].clone()) for b in range(n)]
+            self._self_attn(x, xn, ctx, w, li, st, pos, anc, step_ptr)
+            self._ffn(x, xn, w["n2"], w["ffn"], ACT_RELU)
+        return self._head(x, xn, n)
 
 
 def _pad4(k):
@@ -196,13 +128,15 @@ class _RNNParams(torch.nn.Module):
             torch.nn.init.uniform_(p, -bound, bound)
 
 
-class SequentialRNNLM(torch.nn.Module):
+class SequentialRNNLM(ScorerProtocol, PackedModule):
     """Drop-in container for espnet2.lm.seq_rnn_lm.SequentialRNNLM (inference scorer), LSTM cells only.
 
     One step for n hypotheses is 2L + 3 launches: one gather (embedding row and every layer's parent h into the GEMM operands), per layer one
     GEMM [input | parent h] @ [W_ih | W_hh]^T + (b_ih + b_hh) and one cell kernel, then the output projection and log-softmax.  The recurrent
     state lives in a two-deep ring h, c [2][L][n][Hp] addressed through the search's ancestor table, so it does not grow with the prefix.
     K of every GEMM is padded to a multiple of 4 (TMA needs 16-byte strides) with zero columns in weights and operands."""
+
+    zero_bufs = True   # the operands' pad columns are zeroed when the buffers are created and never written afterwards
 
     def __init__(self, vocab_size: int, unit: int = 650, nhid: int = None, nlayers: int = 2, dropout_rate: float = 0.0, tie_weights: bool = False,
                  rnn_type: str = "lstm", ignore_id: int = 0):
@@ -222,44 +156,22 @@ class SequentialRNNLM(torch.nn.Module):
                 raise ValueError("When using the tied flag, nhid must be equal to emsize")
             self.decoder.weight = self.encoder.weight
         self.vocab_size, self.unit, self.nhid, self.nlayers, self.rnn_type = vocab_size, unit, nhid, nlayers, rnn_type
-        self._packed = None
-        self._ws = {}
-
-    def _load_from_state_dict(self, *args, **kwargs):
-        self._packed = None
-        return super()._load_from_state_dict(*args, **kwargs)
 
     def _pack(self):
-        dev = self.decoder.weight.device
-        f32 = lambda t: t.detach().to(device=dev, dtype=torch.float32)  # noqa: E731
+        f32, dev = self._f32, self._device
         E, H, Ep, Hp = self.unit, self.nhid, _pad4(self.unit), _pad4(self.nhid)
-        pk = dict(emb=f32(self.encoder.weight).contiguous(), layers=[])
+        pk = dict(emb=f32(self.encoder.weight), layers=[])
         for k in range(self.nlayers):
             ip, isz = (Ep, E) if k == 0 else (Hp, H)
             w = torch.zeros(4 * H, ip + Hp, dtype=torch.float32, device=dev)
             w[:, :isz] = f32(getattr(self.rnn, f"weight_ih_l{k}"))
             w[:, ip:ip + H] = f32(getattr(self.rnn, f"weight_hh_l{k}"))
-            pk["layers"].append((split_from(w), (f32(getattr(self.rnn, f"bias_ih_l{k}")) + f32(getattr(self.rnn, f"bias_hh_l{k}"))).contiguous()))
+            pk["layers"].append((split_from(w), f32(getattr(self.rnn, f"bias_ih_l{k}")) + f32(getattr(self.rnn, f"bias_hh_l{k}"))))
         wo = torch.zeros(self.vocab_size, Hp, dtype=torch.float32, device=dev)
         wo[:, :H] = f32(self.decoder.weight)
-        pk["out_w"], pk["out_b"] = split_from(wo), f32(self.decoder.bias).contiguous()
+        pk["out_w"], pk["out_b"] = split_from(wo), f32(self.decoder.bias)
         self._packed = pk
         return pk
-
-    ws_tag = 0
-
-    def _buf(self, name, shape, dtype=torch.float32):
-        """Workspace; zero-filled when (re)created, so that the operands' pad columns are zero (they are never written afterwards)."""
-        name = (self.ws_tag, name)
-        key = (name, tuple(shape), dtype)
-        t = self._ws.get(key)
-        if t is None:
-            for k in [k for k in self._ws if k[0] == name]:
-                del self._ws[k]
-            t = torch.zeros(shape, dtype=dtype, device=self.decoder.weight.device)
-            self._ws[key] = t
-            self.buf_version = getattr(self, "buf_version", 0) + 1   # captured CUDA graphs hold these pointers
-        return t
 
     # ---------------------------------------------------------------- device-side incremental scorer
     @torch.no_grad()
@@ -295,24 +207,10 @@ class SequentialRNNLM(torch.nn.Module):
             _count()
         logp = self._buf("logp", (n, self.vocab_size))
         linear(xo, pk["out_w"], logp, bias=pk["out_b"])
-        from . import ops
-
         ops.log_softmax_rows_(logp)
         return logp
 
     # ---------------------------------------------------------------- BatchScorerInterface (scorer_interface.py:85-188): per hypothesis (h, c)
-    def init_state(self, x: torch.Tensor):
-        return None
-
-    def batch_init_state(self, x: torch.Tensor):
-        return None
-
-    def select_state(self, state, i: int, new_id: int = None):
-        return None if state is None else state[i]
-
-    def final_score(self, state) -> float:
-        return 0.0
-
     @torch.no_grad()
     def batch_score(self, ys: torch.Tensor, states: List[Any], xs: torch.Tensor) -> Tuple[torch.Tensor, List[Any]]:
         """seq_rnn_lm.py:127-166: states per hypothesis (h, c), each [nlayers, nhid], or None at the start (zero state)."""

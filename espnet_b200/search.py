@@ -337,8 +337,8 @@ class _SearchRun:
                 call("espb_transpose_tv_f32", ptr(self.logp_ctc), U, Tmax, V, ptr(self.logp_tok))
                 _count()
         self.side = bs._side_stream(dev, g) if (use_ctc and use_dec) else None
-        self.buf_ver = ((getattr(bs.decoder, "buf_version", 0), id(bs.decoder._packed)) if use_dec else None,
-                        (getattr(bs.lm, "buf_version", 0), id(bs.lm._packed)) if bs.lm is not None else None)
+        self.buf_ver = ((bs.decoder.buf_version, id(bs.decoder._packed)) if use_dec else None,
+                        (bs.lm.buf_version, id(bs.lm._packed)) if bs.lm is not None else None)
 
     def step_body(self, i, cur, sp):
         """One search step. `sp` is None (host step index i) or the device step counter (graph mode: i is ignored)."""
@@ -371,7 +371,7 @@ class _SearchRun:
         logp_dec = None
         if self.use_dec:
             bs.decoder.ws_tag = self.g
-            logp_dec = bs.decoder.step(self.dst, iv, last_tok[cur], anc[cur], W, sp)
+            logp_dec = bs.decoder.step(self.dst, iv, last_tok[cur], anc[cur], sp)
         logp_lm, w_full, logp_full = None, bs.w_dec, logp_dec
         if bs.lm is not None:
             bs.lm.ws_tag = self.g

@@ -20,23 +20,15 @@ from typing import Any, Dict, List, Optional
 
 import torch
 
+from .decoder import ScorerProtocol
 from .search import Hypothesis
 
 
-class LengthBonus:
+class LengthBonus(ScorerProtocol):
     """Constant 1 per emitted token (espnet2/legacy/nets/scorers/length_bonus.py:10-62): weight ``penalty`` in the search."""
 
     def __init__(self, n_vocab: int):
         self.n = n_vocab
-
-    def batch_init_state(self, x):
-        return None
-
-    def select_state(self, state, i, new_id=None):
-        return None if state is None else state[i]
-
-    def final_score(self, state) -> float:
-        return 0.0
 
     def batch_score(self, ys, states, xs):
         return torch.ones(1, dtype=torch.float32, device=ys.device).expand(ys.shape[0], self.n), None
