@@ -20,7 +20,7 @@ from .lm import SequentialRNNLM, TransformerLM, build_lm_from_file  # noqa: F401
 from .search import BatchBeamSearch, Hypothesis  # noqa: F401
 from .search_online import BatchBeamSearchOnline, LengthBonus  # noqa: F401
 from .asr_inference_streaming import Speech2TextStreaming  # noqa: F401
-from .streaming_encoder import ContextualBlockConformerEncoder  # noqa: F401
+from .streaming_encoder import ContextualBlockConformerEncoder, ContextualBlockTransformerEncoder  # noqa: F401
 from .text import TokenIDConverter, build_tokenizer  # noqa: F401
 from .transformer_encoder import TransformerEncoder  # noqa: F401
 

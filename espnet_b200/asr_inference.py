@@ -34,10 +34,10 @@ logger = logging.getLogger(__name__)
 # name -> class registries, as espnet2/tasks/asr.py:95-206 (only the classes on the north-star path)
 frontend_choices = {"default": DefaultFrontend}
 normalize_choices = {"global_mvn": GlobalMVN, "utterance_mvn": UtteranceMVN}
-from .streaming_encoder import ContextualBlockConformerEncoder  # noqa: E402
+from .streaming_encoder import ContextualBlockConformerEncoder, ContextualBlockTransformerEncoder  # noqa: E402
 
 encoder_choices = {"conformer": ConformerEncoder, "transformer": TransformerEncoder, "contextual_block_conformer": ContextualBlockConformerEncoder,
-                   "e_branchformer": EBranchformerEncoder, "branchformer": BranchformerEncoder}
+                   "contextual_block_transformer": ContextualBlockTransformerEncoder, "e_branchformer": EBranchformerEncoder, "branchformer": BranchformerEncoder}
 decoder_choices = {"transformer": TransformerDecoder}
 
 
@@ -142,6 +142,9 @@ class Speech2Text:
         lib.load()  # fail loudly if the CUDA library is missing
         if asr_model is None:
             asr_model, asr_train_args = build_model_from_file(asr_train_config, asr_model_file, device)
+        if isinstance(asr_model.encoder, ContextualBlockTransformerEncoder):
+            raise NotImplementedError("espnet_b200.Speech2Text: the contextual-block Transformer encoder is a streaming encoder (forward_infer "
+                                      "returns no lengths); decode it with Speech2TextStreaming")
         asr_model = asr_model.to(device).eval()
         self.asr_model, self.asr_train_args = asr_model, asr_train_args
         self.device, self.dtype, self.nbest = device, dtype, nbest

@@ -4,7 +4,8 @@
 Reference: espnet2/bin/asr_inference_streaming.py:35-357.  ``apply_frontend`` is the reference's algorithm (waveform overlap buffer of
 (2*ceil(ceil(win/hop)/2) - 1) hops + residual, STFT of the buffered chunk, trimming of the ceil(ceil(win/hop)/2) edge frames) with a leading
 stream dimension: every stream pushes the same number of samples per call, so one (N, n) tensor replaces N Python objects.  The encoder is
-``ContextualBlockConformerEncoder.forward_infer`` (streaming_encoder.py), batched over the streams.
+``ContextualBlockConformerEncoder.forward_infer`` or ``ContextualBlockTransformerEncoder.forward_infer`` (streaming_encoder.py), batched over
+the streams; only its outputs are read, not its lengths (the Transformer returns None there, as the reference).
 
 Decoding: as the reference, every push hands the new encoder frames of a stream to its ``BatchBeamSearchOnline`` (search_online.py: joint CTC /
 attention (/ LM) block-synchronous beam search, one search object per stream, the decoder and LM shared) and returns
