@@ -879,7 +879,17 @@ int espb_glu_dwconv_bn_swish_f32(const float* y, int B, int Tmax, int C, const i
   } else if (!v1 && K == 15) {
     glu_dwconv_bn_swish_win_kernel<15><<<grid, 256, smem_win, stream>>>(y, Tmax, C, lens, dw_w, dw_b, bn_a, bn_b, out, out_plane);
   } else {
+    // tile + weights: 49 408 B at K = 65, 81 152 B at K = 127 -- past the 48 KB a launch gets without opting in
     const size_t smem = ((size_t)(DW_TT + K - 1) * DW_CC + (size_t)DW_CC * K) * sizeof(float);
+    constexpr int smem_max = ((DW_TT + 127 - 1) * DW_CC + DW_CC * 127) * (int)sizeof(float);
+    static bool attr_set = false;
+    if (smem > 48 * 1024 && !attr_set) {
+      if (cudaFuncSetAttribute(glu_dwconv_bn_swish_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max) != cudaSuccess) {
+        espb_set_error("cudaFuncSetAttribute(max dynamic smem) failed (dwconv)");
+        return ESPB_ERR_CUDA;
+      }
+      attr_set = true;
+    }
     glu_dwconv_bn_swish_kernel<<<grid, 256, smem, stream>>>(y, Tmax, C, lens, dw_w, dw_b, K, bn_a, bn_b, out, out_plane);
   }
   ESPB_CHECK_LAUNCH();

@@ -55,6 +55,8 @@ class ConformerEncoder(EncoderBase):
         if not (normalize_before and macaron_style and use_cnn_module) or concat_after: unsupported.append("non pre-LN macaron+cnn block")
         if positionwise_layer_type != "linear" or activation_type != "swish": unsupported.append("positionwise/activation type")
         if zero_triu or qk_norm or len(interctc_layer_idx) or ctc_trim: unsupported.append("zero_triu/qk_norm/interctc/ctc_trim")
+        if cnn_module_kernel < 1 or cnn_module_kernel % 2 == 0 or cnn_module_kernel > 127:
+            unsupported.append(f"cnn_module_kernel={cnn_module_kernel} (odd, <= 127)")
         if unsupported:
             raise NotImplementedError("espnet_b200 ConformerEncoder supports the BASELINE configuration only; got " + ", ".join(unsupported))
         assert output_size % attention_heads == 0

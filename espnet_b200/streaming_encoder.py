@@ -215,6 +215,8 @@ class ContextualBlockConformerEncoder(_ContextualBlockEncoder):
         if positionwise_layer_type != "linear" or activation_type != "swish": bad.append("positionwise / activation type")
         if not init_average or not ctx_pos_enc: bad.append("init_average / ctx_pos_enc = False")
         if block_size <= 0 or hop_size <= 0 or block_size - hop_size - look_ahead < 0: bad.append("block geometry")
+        if cnn_module_kernel < 1 or cnn_module_kernel % 2 == 0 or cnn_module_kernel > 127:
+            bad.append(f"cnn_module_kernel={cnn_module_kernel} (odd, <= 127)")
         if bad:
             raise NotImplementedError("espnet_b200 ContextualBlockConformerEncoder: " + ", ".join(bad))
         assert output_size % attention_heads == 0 and output_size % 32 == 0

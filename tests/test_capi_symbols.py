@@ -111,3 +111,35 @@ def test_transformer_encoder_state_dict_names_match_reference_fixture():
     assert espnet_b200.encoder_choices["transformer"] is espnet_b200.TransformerEncoder
     with pytest.raises(NotImplementedError):
         espnet_b200.TransformerEncoder(80, 64, input_layer="linear")
+
+
+# Entry points the GPU tests reach only through a wrapper, each with the test that runs it.
+COVERED_THROUGH_WRAPPER = {
+    "espb_gemm_f32": "tests/test_gpu_gemm.py::test_linear_plain",                                   # ops.gemm / ops.linear
+    "espb_stft_logmel_f32": "tests/test_gpu_pipeline.py::test_frontend_and_mvn_vs_oracle",          # DefaultFrontend
+    "espb_frontend_blocks": "tests/test_gpu_pipeline.py::test_frontend_and_mvn_vs_oracle",          # DefaultFrontend
+    "espb_utt_mvn_from_partial_f32": "tests/test_gpu_pipeline.py::test_frontend_and_mvn_vs_oracle",  # UtteranceMVN after the frontend
+    "espb_utt_mvn_f32": "tests/test_gpu_pipeline.py::test_standalone_mvn_kernel",                   # UtteranceMVN on its own
+    "espb_global_mvn_f32": "tests/test_gpu_pipeline.py::test_global_mvn_bit_exact_vs_reference_fixture",   # GlobalMVN
+    "espb_abi_version": "tests/test_capi_symbols.py::test_library_exports_every_declared_symbol",    # lib.load
+    "espb_last_error": "tests/test_gpu_encoder_kernels.py::test_layernorm_refuses_D",               # lib.check on a refused call
+}
+
+
+def test_every_entry_point_has_a_gpu_test():
+    """Each espb_* entry point of the header is named in a GPU test file (test_gpu_*.py, or a file with GPU-marked tests), or is on
+    COVERED_THROUGH_WRAPPER with a test that exists."""
+    import glob
+
+    gpu_src = ""
+    for f in sorted(glob.glob(os.path.join(ROOT, "tests", "*.py"))):
+        src = open(f).read()
+        if os.path.basename(f).startswith("test_gpu_") or "pytest.mark.gpu" in src:
+            gpu_src += src
+    named = {s for s in _header_symbols() if re.search(r"\b" + s + r"\b", gpu_src)}
+    uncovered = sorted(set(_header_symbols()) - named - set(COVERED_THROUGH_WRAPPER))
+    assert not uncovered, f"entry points no GPU test calls: {uncovered}"
+    for sym, test in COVERED_THROUGH_WRAPPER.items():
+        assert sym in _header_symbols(), f"{sym} is not in the header any more"
+        path, name = test.split("::")
+        assert re.search(r"^def " + name + r"\(", open(os.path.join(ROOT, path)).read(), flags=re.M), f"{sym}: {test} does not exist"

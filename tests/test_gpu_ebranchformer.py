@@ -77,7 +77,7 @@ def _dw(x, w, b):
     return F.conv1d(x.transpose(1, 2), w.view(C, 1, K), b, padding=(K - 1) // 2, groups=C).transpose(1, 2)
 
 
-@pytest.mark.parametrize("K", [3, 7, 15, 31])
+@pytest.mark.parametrize("K", [3, 7, 15, 31, 63, 127])   # 63 / 127: the run-time-K tile kernel at its widest halo
 @pytest.mark.parametrize("Uh", [96, 200, 1536])
 def test_csgu_kernel_vs_torch(K, Uh):
     from espnet_b200.lib import call, ptr
@@ -101,7 +101,7 @@ def test_csgu_kernel_vs_torch(K, Uh):
         assert bool((out[:, i * T + n:(i + 1) * T] == 0).all())
 
 
-@pytest.mark.parametrize("K", [3, 7, 15, 31])
+@pytest.mark.parametrize("K", [3, 7, 15, 31, 63, 127])   # 63 / 127: the run-time-K tile kernel at its widest halo
 @pytest.mark.parametrize("C2", [128, 200, 1024])
 def test_merge_kernel_vs_torch(K, C2):
     from espnet_b200.lib import call, ptr
