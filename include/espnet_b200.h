@@ -61,18 +61,26 @@ typedef struct EspbGemmDesc {
 int espb_gemm_f32(const EspbGemmDesc* d, int use_tc, cudaStream_t stream);
 
 /* ---- Frontend: Stft.forward + power + LogMel.forward in one kernel ----------------------------------------------
- * espnet2/layers/stft.py:75-120 (torch.stft n_fft 512, hop 128, center/reflect, periodic hann, onesided),
+ * espnet2/layers/stft.py:75-120 (torch.stft n_fft 512, any hop <= 1024, center/reflect, any window, onesided),
  * espnet2/asr/frontend/default.py:110 (re^2+im^2), espnet2/layers/log_mel.py:57-84 (matmul melmat, clamp 1e-10, log,
- * zero padded frames).  wave [B][Lmax], out [B][Tf_max][n_mels], Tf = 1 + len/128.  The mel matrix is passed in the
+ * zero padded frames).  wave [B][Lmax] (utterance b's samples at wave + b*Lmax; samples >= len are not read), out
+ * [B][Tf_max][n_mels], Tf = 1 + len/hop frames per utterance, frames Tf..Tf_max-1 set to 0.  The mel matrix is passed in the
  * sparse form (start/count/offset per filter + packed weights); tw512[k] = (cos, -sin)(2 pi k / 512), k < 256.
- * partial [B][espb_frontend_blocks(Tf_max)][n_mels] receives per-block column sums for the MVN kernel (may be NULL). */
+ * partial [B][espb_frontend_blocks(Tf_max)][n_mels] receives per-block column sums (32 frames per block, frames >= Tf not
+ * counted) for the MVN kernel (may be NULL). */
 int espb_frontend_blocks(int Tf_max);
-/* hop: any hop length (Tf = 1 + len/hop); window: 512 taps (a shorter win_length is zero-padded around the centre by the caller, as torch.stft
- * does); tw256t[k1*16 + n2] = (cos, -sin)(2 pi n2 k1 / 256), the twiddles of the 16 x 16 four-step FFT; mel_nnz = number of packed weights. */
+/* hop: 1..1024 (Tf = 1 + len/hop); window: 512 taps (a shorter win_length is zero-padded around the centre by the caller, as torch.stft
+ * does); tw256t[k1*16 + n2] = (cos, -sin)(2 pi n2 k1 / 256), the twiddles of the 16 x 16 four-step FFT; mel_nnz = number of packed weights
+ * (<= 4096); n_mels <= 128.  Refused with ESPB_ERR_ARG otherwise.  Preconditions the kernel does not check: every length > 256 (the
+ * reflect padding of 256 samples needs them), Tf_max >= 1 + max len / hop, and partial (if not NULL) sized
+ * [B][espb_frontend_blocks(Tf_max)][n_mels]. */
 int espb_stft_logmel_f32(const float* wave, const long long* wave_lens, int B, int Lmax, int hop, const float* window, const float* tw512,
                          const float* tw256t, const int* mel_start, const int* mel_count, const int* mel_offset, const float* mel_weight,
                          int mel_nnz, int n_mels, float* out, int Tf_max, float* partial, cudaStream_t stream);
-/* UtteranceMVN.forward, norm_means only (espnet2/layers/utterance_mvn.py:45-88), in place. */
+/* UtteranceMVN.forward, norm_means only (espnet2/layers/utterance_mvn.py:45-88), in place, n_mels <= 128.  _from_partial takes the
+ * partial sums espb_stft_logmel_f32 wrote for these features (Tf = 1 + wave_len/hop); espb_utt_mvn_f32 computes its own into partial_ws
+ * [B][(Tf_max + 31)/32][n_mels].  Rows t < len get x - mean over those rows; rows t >= len are neither read nor written (the reference
+ * would set them to -mean in a zero-padded batch; every consumer here ignores them). */
 int espb_utt_mvn_from_partial_f32(float* feats, const long long* wave_lens, int B, int Tf_max, int n_mels, int hop, const float* partial,
                                   cudaStream_t stream);
 int espb_utt_mvn_f32(float* feats, const long long* feat_lens, int B, int Tf_max, int n_mels, float* partial_ws, cudaStream_t stream);
@@ -114,7 +122,12 @@ int espb_masked_softmax_f32(const float* scores, int B, int H, int T, int Tp, co
  * out[b,i,h,:] = softmax_j<len_b( (q[b,i,h,:] . k[b,j,h,:] + bd[b,h,i,T-1-i+j]) / sqrt(d_k) ) . v[b,j,h,:].
  * q / k / out are split (hi/lo plane) tensors (first element at q + q_off / k + k_off) with row strides ldq / ldk / ldo, head h at columns h*64..; vt is the split V^T [B][H][64][Tp]
  * written by espb_v_transpose_f32; bd is the UNSHIFTED (q + pos_bias_v) p^T product [B][H][T][Rp] (rel_shift is applied while loading) or NULL
- * for absolute-position attention.  Replaces the q k^T GEMM + espb_relpos_softmax_f32 / espb_masked_softmax_f32 + p v GEMM sequence. */
+ * for absolute-position attention.  Replaces the q k^T GEMM + espb_relpos_softmax_f32 / espb_masked_softmax_f32 + p v GEMM sequence.
+ * vt must hold zeros at keys >= len (espb_v_transpose_f32 writes them): those keys get weight 0, and 0 * NaN would not be 0.  Only keys
+ * < len of k and only the band columns T-1-i .. T-1-i+len-1 of bd row i are read.  An utterance with len = 0 gets an all-zero output, as
+ * does every 128-query block that starts at or beyond len; query rows len <= t < T of a block that also holds valid rows are finite.
+ * d_k must be 64, B, H, T > 0; ldq, q_plane, ldo, out_plane multiples of 4 and q, out 16-byte aligned; ldk, k_plane, vt_plane and
+ * Tp multiples of 4 (TMA strides).  Refused with ESPB_ERR_ARG / ESPB_ERR_TMA otherwise. */
 int espb_flash_attn_f32(const float* q, long long q_off, long long q_plane, long long ldq, const float* k, long long k_off, long long k_plane,
                         long long ldk, const float* vt, long long vt_plane, int Tp, const float* bd, int Rp, const int* lens, int B, int H, int T,
                         int dk, float* out, long long out_plane, long long ldo, cudaStream_t stream);

@@ -116,11 +116,6 @@ def test_transformer_encoder_state_dict_names_match_reference_fixture():
 # Entry points the GPU tests reach only through a wrapper, each with the test that runs it.
 COVERED_THROUGH_WRAPPER = {
     "espb_gemm_f32": "tests/test_gpu_gemm.py::test_linear_plain",                                   # ops.gemm / ops.linear
-    "espb_stft_logmel_f32": "tests/test_gpu_pipeline.py::test_frontend_and_mvn_vs_oracle",          # DefaultFrontend
-    "espb_frontend_blocks": "tests/test_gpu_pipeline.py::test_frontend_and_mvn_vs_oracle",          # DefaultFrontend
-    "espb_utt_mvn_from_partial_f32": "tests/test_gpu_pipeline.py::test_frontend_and_mvn_vs_oracle",  # UtteranceMVN after the frontend
-    "espb_utt_mvn_f32": "tests/test_gpu_pipeline.py::test_standalone_mvn_kernel",                   # UtteranceMVN on its own
-    "espb_global_mvn_f32": "tests/test_gpu_pipeline.py::test_global_mvn_bit_exact_vs_reference_fixture",   # GlobalMVN
     "espb_abi_version": "tests/test_capi_symbols.py::test_library_exports_every_declared_symbol",    # lib.load
     "espb_last_error": "tests/test_gpu_encoder_kernels.py::test_layernorm_refuses_D",               # lib.check on a refused call
 }
