@@ -3,7 +3,7 @@
 Public surface mirrors the reference classes on that path (see SURVEY.md section 8b):
 Speech2Text, ESPnetASRModel, DefaultFrontend, UtteranceMVN, ConformerEncoder, CTC,
 TransformerDecoder, BatchBeamSearch, Hypothesis, TooShortUttError (+ GlobalMVN, the output-side text classes, and the
-TransformerEncoder of the next scope row, the EBranchformerEncoder and the BranchformerEncoder; CTCPrefixScorer and TransformerDecoder.batch_score implement the reference's scorer protocol,
+TransformerEncoder of the next scope row, the EBranchformerEncoder and the BranchformerEncoder, the RNN family's VGGRNNEncoder, RNNEncoder and RNNDecoder; CTCPrefixScorer and TransformerDecoder.batch_score implement the reference's scorer protocol,
 ``espnet_b200.integration.register()`` adds the classes to the reference's registries).
 All compute goes through the C-ABI CUDA library ``libespnet_b200.so`` (include/espnet_b200.h).
 """
@@ -16,6 +16,8 @@ from .e_branchformer_encoder import EBranchformerEncoder  # noqa: F401
 from .encoder import ConformerEncoder  # noqa: F401
 from .errors import TooShortUttError  # noqa: F401
 from .frontend import DefaultFrontend, GlobalMVN, LogMel, UtteranceMVN  # noqa: F401
+from .rnn_decoder import RNNDecoder  # noqa: F401
+from .rnn_encoder import RNNEncoder, VGGRNNEncoder  # noqa: F401
 from .lm import SequentialRNNLM, TransformerLM, build_lm_from_file  # noqa: F401
 from .search import BatchBeamSearch, Hypothesis  # noqa: F401
 from .search_online import BatchBeamSearchOnline, LengthBonus  # noqa: F401

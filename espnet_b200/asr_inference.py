@@ -26,6 +26,8 @@ from .encoder import ConformerEncoder
 from .errors import TooShortUttError  # noqa: F401
 from .frontend import DefaultFrontend, GlobalMVN, UtteranceMVN
 from .text import TokenIDConverter, tokenizer_for_inference
+from .rnn_decoder import RNNDecoder
+from .rnn_encoder import RNNEncoder, VGGRNNEncoder
 from .search import BatchBeamSearch, Hypothesis
 from .transformer_encoder import TransformerEncoder
 
@@ -37,8 +39,9 @@ normalize_choices = {"global_mvn": GlobalMVN, "utterance_mvn": UtteranceMVN}
 from .streaming_encoder import ContextualBlockConformerEncoder, ContextualBlockTransformerEncoder  # noqa: E402
 
 encoder_choices = {"conformer": ConformerEncoder, "transformer": TransformerEncoder, "contextual_block_conformer": ContextualBlockConformerEncoder,
-                   "contextual_block_transformer": ContextualBlockTransformerEncoder, "e_branchformer": EBranchformerEncoder, "branchformer": BranchformerEncoder}
-decoder_choices = {"transformer": TransformerDecoder}
+                   "contextual_block_transformer": ContextualBlockTransformerEncoder, "e_branchformer": EBranchformerEncoder, "branchformer": BranchformerEncoder,
+                   "vgg_rnn": VGGRNNEncoder, "rnn": RNNEncoder}
+decoder_choices = {"transformer": TransformerDecoder, "rnn": RNNDecoder}
 
 
 class ESPnetASRModel(torch.nn.Module):

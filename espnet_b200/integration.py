@@ -15,8 +15,10 @@ NAMES = {"frontend": {"b200_default": "DefaultFrontend"},
          "encoder": {"b200_conformer": "ConformerEncoder", "b200_transformer": "TransformerEncoder",
                      "b200_contextual_block_conformer": "ContextualBlockConformerEncoder",
                      "b200_contextual_block_transformer": "ContextualBlockTransformerEncoder", "b200_e_branchformer": "EBranchformerEncoder",
-                     "b200_branchformer": "BranchformerEncoder"},
-         "decoder": {"b200_transformer": "TransformerDecoder"}}
+                     "b200_branchformer": "BranchformerEncoder", "b200_vgg_rnn": "VGGRNNEncoder", "b200_rnn": "RNNEncoder"},
+         "decoder": {"b200_transformer": "TransformerDecoder", "b200_rnn": "RNNDecoder"}}
+# decoders that implement the reference's non-batch ScorerInterface only (the reference's Speech2Text then builds its BeamSearch)
+_NON_BATCH = {"RNNDecoder"}
 
 
 def _derive(name, base, *abcs, extra=None):
@@ -32,10 +34,10 @@ def register():
     from espnet2.asr.encoder.abs_encoder import AbsEncoder
     from espnet2.asr.frontend.abs_frontend import AbsFrontend
     from espnet2.layers.abs_normalize import AbsNormalize
-    from espnet2.legacy.nets.scorer_interface import BatchScorerInterface
+    from espnet2.legacy.nets.scorer_interface import BatchScorerInterface, ScorerInterface
 
     def _no_training_forward(self, hs_pad, hlens, ys_in_pad, ys_in_lens):
-        raise NotImplementedError("espnet_b200.TransformerDecoder is an inference scorer (batch_score); the training forward is not on this path")
+        raise NotImplementedError(f"espnet_b200.{type(self).__name__} is an inference scorer; the training forward is not on this path")
 
     bases = {"frontend": (AbsFrontend,), "normalize": (AbsNormalize,), "encoder": (AbsEncoder,), "decoder": (AbsDecoder, BatchScorerInterface)}
     added = {}
@@ -44,7 +46,8 @@ def register():
         for choice, cls_name in names.items():
             if choice not in choices.classes:
                 extra = {"forward": _no_training_forward} if reg == "decoder" else None
-                choices.classes[choice] = _derive(cls_name, getattr(espnet_b200, cls_name), *bases[reg], extra=extra)
+                abcs = (AbsDecoder, ScorerInterface) if cls_name in _NON_BATCH else bases[reg]
+                choices.classes[choice] = _derive(cls_name, getattr(espnet_b200, cls_name), *abcs, extra=extra)
             added.setdefault(reg, {})[choice] = choices.classes[choice]
     return added
 

@@ -83,6 +83,12 @@ _SIGS = {
     "espb_count_active_i32": [P, I, P, P],
     "espb_rnnlm_gather_f32": [P, P, I, I, P, I, I, P, P, I, I, I, I, P, P],
     "espb_lstm_cell_f32": [P, P, I, I, P, P, P, I, I, I, I, I, P, L, I, P],
+    "espb_vgg_conv1_relu_f32": [P, I, I, I, P, P, P, I, P, I, P],
+    "espb_vgg_pool_f32": [P, I, I, I, I, P, I, I, P, L, P],
+    "espb_lstm_rec_step_f32": [P, P, P, I, I, I, I, I, I, P, L, P, P, L, I, P],
+    "espb_rnn_proj_post_f32": [P, I, I, I, P, I, I, P, L, I, P],
+    "espb_drop_cand_i32": [P, I, I, I, P],
+    "espb_att_loc_step_f32": [P, P, L, P, I, I, I, I, P, P, I, I, P, P, P, P, I, I, P, P, I, P, L, I, P, L, I, P],
 }
 
 ABI_VERSION = 7   # espb_abi_version() of the library this binding matches (include/espnet_b200.h)

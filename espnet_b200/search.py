@@ -387,6 +387,11 @@ class _SearchRun:
             call("espb_ctc_score_cands_f32", ptr(self.logp_tok), U, Tmax, V, ptr(lens32), 0, bs.eos, W, ptr(r[cur]), ptr(s_prev[cur]),
                  ptr(last_tok[cur]), iv, ptr(sp), ptr(st["cand_ids"]), P, ptr(st["part"]), ptr(st["psi"]), ptr(st["valid"]), self.tok_major)
             _count()
+            if getattr(bs.decoder, "eos_from_prebeam_only", False):
+                # the reference decodes such a decoder with its non-batch BeamSearch (beam_search.py:347-361), where <eos> competes only when
+                # the pre-beam holds it: the appended <eos> candidate P is dropped
+                call("espb_drop_cand_i32", ptr(st["valid"]), n, P + 1, P)
+                _count()
         elif mode == 0:
             ops.rows_topk(logp_full, w_full, P, st["cand_ids"], st["cand_val"])
         else:

@@ -239,6 +239,41 @@ int espb_rnnlm_gather_f32(const int* tok, const float* emb, int E, int Ep, const
    into the ring; h' also split into out[s*out_ld + j] (plane out_plane): the next layer's input half or the output projection's operand */
 int espb_lstm_cell_f32(const float* gates, const int* anc, int anc_ld, int pos, const int* step_ptr, float* h_ring, float* c_ring, int layer, int L,
                        int n, int H, int Hp, float* out, long long out_plane, int out_ld, cudaStream_t stream);
+/* ---- RNN model family (espnet2/asr/encoder/vgg_rnn_encoder.py, rnn_encoder.py, legacy/nets/pytorch_backend/rnn/encoders.py,
+ *      asr/decoder/rnn_decoder.py, rnn/attentions.py AttLoc).  The GEMMs (VGG convs as implicit GEMM a_mode 2 over zero-bordered inputs,
+ *      input-to-gate products, h W_hh^T, projections, mlp_enc / mlp_dec, decoder gates and output) run on espb_gemm_f32. ---- */
+/* VGG2L conv1_1 + ReLU: feats [B][Tf_max][F], utterance b seeing zeros at t >= lens[b] -> split [B][2][F+2][T+2][C] with a zero border
+ * and zero rows t >= lens[b] (the input of conv1_2 as implicit GEMM).  w [C][9] ((kt, kf) order), C <= 256. */
+int espb_vgg_conv1_relu_f32(const float* feats, int B, int Tf_max, int F, const int* lens, const float* w, const float* bias, int C, float* out,
+                            int T, cudaStream_t stream);
+/* VGG2L conv output x [B][F][T][C] (plain, ReLU applied), valid at t < lens[b] -> optional 2x2 ceil-mode max-pool over the valid rows
+ * (pool = 1: Fo = ceil(F/2), To = ceil(T/2), new length ceil(len/2)) -> flat = 0: split [B][2][Fo+2][To+2][C] zero-bordered (planes
+ * out_plane = (Fo+2)(To+2)C apart within an utterance's block); flat = 1: split rows [B*To][C*Fo], column c*Fo + f (the reference's
+ * (channel, freq) flattening), planes out_plane apart.  Rows at or past the new length are 0. */
+int espb_vgg_pool_f32(const float* x, int B, int F, int T, int C, const int* lens, int pool, int flat, float* out, long long out_plane,
+                      cudaStream_t stream);
+/* Step s of a 1-layer (B)LSTM over B utterances (packed-sequence semantics): direction d handles frame s (d = 0) or lens[b]-1-s (d = 1).
+ * xg [B][T][ndir*4H] input gates with both biases, hg [ndir][B][4H] = h W_hh^T of the previous step (not read at s = 0, where h = c = 0);
+ * h' -> h split [2][ndir][B][Hp] (planes h_plane apart), c' -> c [ndir][B][H], h' -> y split [B][T][ldy] columns d*H..; at s >= lens[b]
+ * y[b][s] is set to 0 in both directions.  Gate order i, f, g, o; expf / tanhf. */
+int espb_lstm_rec_step_f32(const float* xg, const float* hg, const int* lens, int s, int B, int T, int H, int Hp, int ndir, float* h,
+                           long long h_plane, float* c, float* y, long long y_plane, int ldy, cudaStream_t stream);
+/* Projection epilogue: x [B][T][D] plain -> tanh (act = 1) or identity, rows t >= lens[b] set to 0, into x (write_plain) and / or split
+ * into out [B*T][ldo] (out may be NULL). */
+int espb_rnn_proj_post_f32(float* x, int B, int T, int D, const int* lens, int act, int write_plain, float* out, long long out_plane, int ldo,
+                           cudaStream_t stream);
+/* AttLoc step for n = U*W slots (slot s belongs to utterance s / W): previous weights from ring [2][n][Tmax] at (pos-1)&1, slot
+ * anc[s*anc_ld + pos-1] (uniform 1/len at pos 0), loc conv (conv_w [chans][2 filts + 1]) + mlp_att (att_wt [chans][A], transposed),
+ * e = gvec . tanh(loc + enc_h[u][t] + dec_z[s]) + gvec_b, masked softmax(2 e) over t < lens[u] -> ring[pos&1][s] (0 past len), context
+ * sum_t w_t enc[u][t] (enc split [U][Tmax][E], hi + lo) split into out[s*out_ld ..] and, if not NULL, out2[s*out2_ld ..].  enc_h [U][Tmax][A]
+ * = mlp_enc(enc).  One block per slot; refused when (Tmax + 2 filts + chans Tmax + Tmax + chans A + 33) floats exceed 227 KiB. */
+int espb_att_loc_step_f32(const float* enc_h, const float* enc, long long enc_plane, const int* lens, int W, int Tmax, int A, int E,
+                          const float* dec_z, const float* conv_w, int chans, int filts, const float* att_wt, const float* gvec,
+                          const float* gvec_b, const int* anc, int anc_ld, int pos, const int* step_ptr, float* ring, int n, float* out,
+                          long long out_plane, int out_ld, float* out2, long long out2_plane, int out2_ld, cudaStream_t stream);
+/* valid[s*PC + j] = 0 for every slot s < n: drops candidate j (the appended <eos> of espb_ctc_score_cands_f32) for decoders the reference
+ * decodes with its non-batch BeamSearch, where <eos> competes only from within the pre-beam (beam_search.py:347-361). */
+int espb_drop_cand_i32(int* valid, int n, int PC, int j, cudaStream_t stream);
 int espb_step_inc_i32(int* step, cudaStream_t stream);
 int espb_count_active_i32(const int* active, int n, int* out, cudaStream_t stream);
 
