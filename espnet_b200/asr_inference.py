@@ -53,6 +53,8 @@ class ESPnetASRModel(torch.nn.Module):
         self.sos = self.eos = vocab_size - 1  # espnet_model.py:76-87
         self.vocab_size, self.token_list = vocab_size, list(token_list)
         self.frontend, self.normalize, self.encoder = frontend, normalize, encoder
+        if getattr(encoder, "interctc_use_conditioning", False):   # espnet_model.py:104-107 (self-conditioned intermediate CTC)
+            encoder.conditioning_layer = torch.nn.Linear(vocab_size, encoder.output_size())
         self.decoder = decoder
         self.ctc = ctc
         self.ctc_weight = ctc_weight
@@ -64,7 +66,12 @@ class ESPnetASRModel(torch.nn.Module):
         feats, feats_lengths = self.frontend(speech, speech_lengths)
         if self.normalize is not None:
             feats, feats_lengths = self.normalize(feats, feats_lengths)
-        enc, enc_lens, _ = self.encoder(feats, feats_lengths)
+        if getattr(self.encoder, "interctc_use_conditioning", False):   # espnet_model.py:412-425
+            enc, enc_lens, _ = self.encoder(feats, feats_lengths, ctc=self.ctc)
+        else:
+            enc, enc_lens, _ = self.encoder(feats, feats_lengths)
+        if isinstance(enc, tuple):   # (output, intermediate outputs): decoding uses the output only (asr_inference.py: enc[0])
+            enc = enc[0]
         return enc, enc_lens
 
     def enc_split(self, enc):

@@ -1,6 +1,7 @@
-// CTC head kernels: row-wise log-softmax / argmax over the vocabulary and on-device greedy collapse.
-// Reference: espnet2/asr/ctc.py:197-215 (log_softmax, argmax), espnet2/bin/asr_inference.py:574-575 and
-// espnet2/bin/s2t_inference_ctc.py:630-632 (unique_consecutive + drop blank).
+// CTC head kernels: row-wise log-softmax / argmax over the vocabulary, on-device greedy collapse, and the row softmax that feeds the
+// self-conditioning GEMM of intermediate CTC.
+// Reference: espnet2/asr/ctc.py:187-215 (softmax, log_softmax, argmax), espnet2/asr/encoder/conformer_encoder.py:394-414 (conditioning),
+// espnet2/bin/asr_inference.py:574-575 and espnet2/bin/s2t_inference_ctc.py:630-632 (unique_consecutive + drop blank).
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -49,6 +50,69 @@ __global__ void __launch_bounds__(256) log_softmax_rows_reg_kernel(float* __rest
     const int i = threadIdx.x + k * 256;
     if (i < V) r[i] = v[k] - lse;
   }
+}
+
+// Softmax of each row of x [rows][V] (row pitch ld) into the tf32 hi / lo planes out, out + out_plane [rows][ldo] (the A operand of the
+// 3xTF32 GEMM), columns V..ldo-1 zero. One block per row; the same per-thread summation order as log_softmax_rows_reg_kernel, with
+// x[t + 256 k], k < NV, held in registers (V <= 256 NV).
+__device__ __forceinline__ void store_split_row(float* __restrict__ o, long long plane, int i, float p) {
+  const float hi = espb::tf32_hi(p);
+  o[i] = hi;
+  o[plane + i] = espb::tf32_lo(p, hi);
+}
+
+__device__ __forceinline__ void zero_split_tail(float* __restrict__ o, long long plane, int V, long long ldo) {
+  for (long long i = V + threadIdx.x; i < ldo; i += blockDim.x) { o[i] = 0.f; o[plane + i] = 0.f; }
+}
+
+template <int NV>
+__global__ void __launch_bounds__(256) softmax_rows_split_reg_kernel(const float* __restrict__ x, long long ld, int V, float* __restrict__ out,
+                                                                     long long out_plane, long long ldo) {
+  espb::pdl_trigger();
+  espb::pdl_wait();
+  __shared__ float red[33];
+  const float* r = x + (long long)blockIdx.x * ld;
+  float* o = out + (long long)blockIdx.x * ldo;
+  float v[NV];
+  float mx = -INFINITY;
+#pragma unroll
+  for (int k = 0; k < NV; ++k) {
+    const int i = threadIdx.x + k * 256;
+    v[k] = (i < V) ? r[i] : -INFINITY;
+    mx = fmaxf(mx, v[k]);
+  }
+  mx = espb::block_max(mx, red);
+  float s = 0.f;
+#pragma unroll
+  for (int k = 0; k < NV; ++k) {
+    v[k] = expf(v[k] - mx);
+    if (threadIdx.x + k * 256 < V) s += v[k];
+  }
+  s = espb::block_sum(s, red);
+#pragma unroll
+  for (int k = 0; k < NV; ++k) {
+    const int i = threadIdx.x + k * 256;
+    if (i < V) store_split_row(o, out_plane, i, v[k] / s);
+  }
+  zero_split_tail(o, out_plane, V, ldo);
+}
+
+// Same result for any V: three passes over the row in global memory (max, sum, store), each thread visiting the same columns in the same order.
+__global__ void __launch_bounds__(256) softmax_rows_split_kernel(const float* __restrict__ x, long long ld, int V, float* __restrict__ out,
+                                                                 long long out_plane, long long ldo) {
+  espb::pdl_trigger();
+  espb::pdl_wait();
+  __shared__ float red[33];
+  const float* r = x + (long long)blockIdx.x * ld;
+  float* o = out + (long long)blockIdx.x * ldo;
+  float mx = -INFINITY;
+  for (int i = threadIdx.x; i < V; i += 256) mx = fmaxf(mx, r[i]);
+  mx = espb::block_max(mx, red);
+  float s = 0.f;
+  for (int i = threadIdx.x; i < V; i += 256) s += expf(r[i] - mx);
+  s = espb::block_sum(s, red);
+  for (int i = threadIdx.x; i < V; i += 256) store_split_row(o, out_plane, i, expf(r[i] - mx) / s);
+  zero_split_tail(o, out_plane, V, ldo);
 }
 
 // argmax of each row (first index on ties, as torch.argmax on CPU). One warp per row.
@@ -105,6 +169,22 @@ int espb_log_softmax_rows_f32(float* x, long long rows, long long ld, int V, cud
   else if (!three_pass && V <= 256 * 20) espb::launch_pdl(log_softmax_rows_reg_kernel<20>, dim3((unsigned)rows), dim3(256), 0, stream, x, ld, V);
   else if (!three_pass && V <= 256 * 32) espb::launch_pdl(log_softmax_rows_reg_kernel<32>, dim3((unsigned)rows), dim3(256), 0, stream, x, ld, V);
   else espb::launch_pdl(log_softmax_rows_kernel, dim3((unsigned)rows), dim3(256), 0, stream, x, ld, V);
+  ESPB_CHECK_LAUNCH();
+  return ESPB_OK;
+}
+
+int espb_softmax_rows_split_f32(const float* x, long long rows, long long ld, int V, float* out, long long out_plane, long long ldo,
+                                cudaStream_t stream) {
+  if (rows < 0 || V <= 0 || ld < V) { espb_set_error("softmax_rows_split: need rows >= 0, V > 0 and ld >= V"); return ESPB_ERR_ARG; }
+  if (ldo < V || ldo % 32) { espb_set_error("softmax_rows_split: ldo must be a multiple of 32 and >= V"); return ESPB_ERR_ARG; }
+  if (out_plane < rows * ldo) { espb_set_error("softmax_rows_split: out_plane must be >= rows * ldo"); return ESPB_ERR_ARG; }
+  if (rows == 0) return ESPB_OK;
+  if (!x || !out) { espb_set_error("softmax_rows_split: null pointer"); return ESPB_ERR_ARG; }
+  const dim3 grid((unsigned)rows), block(256);
+  if (V <= 256 * 8) espb::launch_pdl(softmax_rows_split_reg_kernel<8>, grid, block, 0, stream, x, ld, V, out, out_plane, ldo);
+  else if (V <= 256 * 20) espb::launch_pdl(softmax_rows_split_reg_kernel<20>, grid, block, 0, stream, x, ld, V, out, out_plane, ldo);
+  else if (V <= 256 * 32) espb::launch_pdl(softmax_rows_split_reg_kernel<32>, grid, block, 0, stream, x, ld, V, out, out_plane, ldo);
+  else espb::launch_pdl(softmax_rows_split_kernel, grid, block, 0, stream, x, ld, V, out, out_plane, ldo);
   ESPB_CHECK_LAUNCH();
   return ESPB_OK;
 }

@@ -5,12 +5,13 @@ Reference: espnet2/asr/encoder/conformer_encoder.py:89-429 and the legacy module
 (Conv2dSubsampling, RelPositionalEncoding, EncoderLayer, RelPositionMultiHeadedAttention,
 PositionwiseFeedForward, ConvolutionModule, LayerNorm).  Supported configuration = the one
 BASELINE.json names, with input_layer "conv2d", "conv2d2", "conv2d6" or "conv2d8"; rel_pos_type "latest" (rel_pos / rel_selfattn),
-macaron_style, use_cnn_module, swish, normalize_before, no intermediate CTC.  The subsampling, FFN,
-rel-pos self-attention and convolution module are the shared ones of layers.py.  The torch.nn layers
+macaron_style, use_cnn_module, swish, normalize_before, intermediate CTC with or without self-conditioning
+(interctc_layer_idx / interctc_use_conditioning; no ctc_trim).  The subsampling, FFN, rel-pos self-attention, convolution module and
+intermediate-CTC step are the shared ones of layers.py.  The torch.nn layers
 are parameter containers only (so that reference checkpoints load by name); forward never calls them.
 """
 import math
-from typing import List, Optional, Tuple, Union
+from typing import List, Optional, Union
 
 import torch
 
@@ -54,7 +55,7 @@ class ConformerEncoder(EncoderBase):
             unsupported.append("rel_pos_type/pos_enc_layer_type/selfattention_layer_type other than latest/rel_pos/rel_selfattn")
         if not (normalize_before and macaron_style and use_cnn_module) or concat_after: unsupported.append("non pre-LN macaron+cnn block")
         if positionwise_layer_type != "linear" or activation_type != "swish": unsupported.append("positionwise/activation type")
-        if zero_triu or qk_norm or len(interctc_layer_idx) or ctc_trim: unsupported.append("zero_triu/qk_norm/interctc/ctc_trim")
+        if zero_triu or qk_norm or ctc_trim: unsupported.append("zero_triu/qk_norm/ctc_trim")
         if cnn_module_kernel < 1 or cnn_module_kernel % 2 == 0 or cnn_module_kernel > 127:
             unsupported.append(f"cnn_module_kernel={cnn_module_kernel} (odd, <= 127)")
         if unsupported:
@@ -65,6 +66,7 @@ class ConformerEncoder(EncoderBase):
         super().__init__(input_size, output_size,
                          (_EncoderLayer(output_size, attention_heads, linear_units, cnn_module_kernel) for _ in range(num_blocks)), input_layer)
         self.heads, self.num_blocks, self.kernel = attention_heads, num_blocks, cnn_module_kernel
+        self._init_interctc(interctc_layer_idx, interctc_use_conditioning, num_blocks)
 
     def _pack(self):
         pk = self._pack_io()
@@ -80,12 +82,14 @@ class ConformerEncoder(EncoderBase):
         return pk
 
     @torch.no_grad()
-    def forward(self, xs_pad: torch.Tensor, ilens: torch.Tensor, prev_states: torch.Tensor = None
-                ) -> Tuple[torch.Tensor, torch.Tensor, Optional[torch.Tensor]]:
-        """xs_pad (B, T_f, idim) float32 CUDA (normalised log-mel), ilens (B,) -> (B, T, D), olens, None.
+    def forward(self, xs_pad: torch.Tensor, ilens: torch.Tensor, prev_states: torch.Tensor = None, ctc=None):
+        """xs_pad (B, T_f, idim) float32 CUDA (normalised log-mel), ilens (B,) -> (B, T, D), olens, None; with interctc_layer_idx
+        ((B, T, D), [(layer, after_norm of that block's output), ...]), olens, None.  ctc: the CTC head, needed with
+        interctc_use_conditioning.
 
         Ragged batches follow per-utterance (batch-1) semantics of the reference: every utterance sees only
         its own frames (own conv boundaries, own attention keys); rows t >= olens[b] of the output are padding."""
+        self._check_interctc(ctc)
         pk = self._packed or self._pack()
         xs_pad, T, olens, lens32 = self._lengths(xs_pad, ilens)   # check_short_utt: conformer_encoder.py:363-371
         B, D = xs_pad.shape[0], self._output_size
@@ -96,6 +100,7 @@ class ConformerEncoder(EncoderBase):
             self.trace.append(x.view(B, T, D).clone())
         p_all = self._pos(T)
         xn, qkv, ctx = self._buf("xn", (2, M, D)), self._buf("qkv", (2, M, 3 * D)), self._buf("ctx", (2, M, D))
+        inter = []
         for li, w in enumerate(pk["layers"]):
             # macaron FFN: x += 0.5 * w2(swish(w1(LN(x))))   (encoder_layer.py:115-123)
             self._ffn(x, xn, w["norm_ff_macaron"], w["feed_forward_macaron"], ACT_SWISH, 0.5)
@@ -111,5 +116,7 @@ class ConformerEncoder(EncoderBase):
             layernorm(x, *w["norm_final"], LN_EPS, out_plain=x)
             if self.trace is not None:
                 self.trace.append(x.view(B, T, D).clone())
+            if li + 1 in self.interctc_layer_idx:
+                inter.append((li + 1, self._interctc(x, B, T, ctc)))
         out, _ = self._output(x, B, T)
-        return out, olens, None
+        return ((out, inter) if inter else out), olens, None

@@ -218,6 +218,28 @@ class EncoderBase(PackedModule):
     def output_size(self) -> int:
         return self._output_size
 
+    def _init_interctc(self, interctc_layer_idx, interctc_use_conditioning, num_blocks):
+        """Intermediate CTC (conformer_encoder.py:317-321): after each listed block (1-based) the encoder returns after_norm(x) and, with
+        conditioning, feeds the CTC posteriors back into x through ``conditioning_layer``, which ESPnetASRModel creates."""
+        self.interctc_layer_idx = list(interctc_layer_idx)
+        if len(self.interctc_layer_idx) > 0:
+            assert 0 < min(self.interctc_layer_idx) and max(self.interctc_layer_idx) < num_blocks
+        self.interctc_use_conditioning = interctc_use_conditioning
+        self.conditioning_layer = None
+
+    def _check_interctc(self, ctc):
+        if self.interctc_layer_idx and self.interctc_use_conditioning:
+            if ctc is None:
+                raise ValueError(f"{type(self).__name__} with interctc_use_conditioning needs the CTC head: call it as encoder(xs_pad, ilens, "
+                                 "ctc=model.ctc)")
+            if self.conditioning_layer is None:
+                raise ValueError(f"{type(self).__name__} with interctc_use_conditioning has no conditioning_layer: ESPnetASRModel creates it "
+                                 "(Linear(vocab_size, output_size))")
+            if self.conditioning_layer.in_features != ctc.odim:
+                raise ValueError(f"conditioning_layer takes {self.conditioning_layer.in_features} posteriors, the CTC head has {ctc.odim}")
+            if self._packed is not None and "cond_w" not in self._packed:   # conditioning_layer set after the weights were packed
+                self._packed = None
+
     def _pack_pos(self, attns):
         """linear_pos of every attention layer stacked [L*D][D], L = the number of attention layers (layer ordinal a at rows a*D..): one GEMM
         per length projects the rel-pos table for all of them (_pos)."""
@@ -242,7 +264,7 @@ class EncoderBase(PackedModule):
         return d
 
     def _pack_io(self):
-        """Conv2dSubsampling in the layouts of the conv1 kernel and the implicit-GEMM convs, and after_norm."""
+        """Conv2dSubsampling in the layouts of the conv1 kernel and the implicit-GEMM convs, after_norm, and conditioning_layer if set."""
         f32, e = self._f32, self.embed
         D = C = self._output_size
         Fs = subsampled_len(self.idim, self.input_layer)
@@ -254,7 +276,17 @@ class EncoderBase(PackedModule):
         return dict(F=Fs, c1_w=f32(e.conv[0].weight).view(C, 9), c1_b=f32(e.conv[0].bias), convs=convs,
                     # embed.out columns are c*F+f (subsampling.py:450-451) -> f*C+c to match the [B][F][T][C] output of the last conv
                     out_w=split_from(f32(e.out.weight).view(D, C, Fs[-1]).permute(0, 2, 1).reshape(D, Fs[-1] * C)), out_b=f32(e.out.bias),
-                    after_norm=self._pack_ln(self.after_norm))
+                    after_norm=self._pack_ln(self.after_norm), **self._pack_cond())
+
+    def _pack_cond(self):
+        """conditioning_layer [D][V] as the B operand of a GEMM with K = _pitch(V): zero columns V.. meet the zero columns of the posteriors."""
+        cl = getattr(self, "conditioning_layer", None)
+        if cl is None:
+            return {}
+        w = self._f32(cl.weight)
+        wp = torch.zeros(w.shape[0], _pitch(w.shape[1]), dtype=torch.float32, device=w.device)
+        wp[:, : w.shape[1]] = w
+        return dict(cond_w=split_from(wp), cond_b=self._f32(cl.bias))
 
     # ---------------------------------------------------------------- launches
     def _lengths(self, xs_pad, ilens):
@@ -400,6 +432,25 @@ class EncoderBase(PackedModule):
             _count()
             ops.gemm(S, dk, S, probs, nseq * H * S * Sp, Sp, vt, nseq * H * dk * Sp, Sp, ctx, D, c_plane=M * D, split_out=True, nbx=H, nby=nseq,
                      sa=(S * Sp, H * S * Sp), sb=(dk * Sp, H * dk * Sp), sc=(dk, S * D))
+
+    def _interctc(self, x, B, T, ctc):
+        """After a block listed in interctc_layer_idx (conformer_encoder.py:391-414, transformer_encoder.py:279-291): returns the intermediate
+        output after_norm(x) as a new (B, T, D) tensor and, with conditioning, adds conditioning_layer(softmax(ctc_lo(after_norm(x)))) to x.
+        The posteriors go straight into the split A operand of the conditioning GEMM, zero-padded to a K that is a multiple of 32.  Every
+        step is row-wise, so padding rows of a ragged batch only reach padding rows."""
+        D, M = self._output_size, B * T
+        h = torch.empty(B, T, D, dtype=torch.float32, device=x.device)
+        if not self.interctc_use_conditioning:
+            layernorm(x, *self._packed["after_norm"], LN_EPS, out_plain=h)
+            return h
+        V = ctc.odim
+        hs = self._buf("ic_split", (2, M, D))
+        logits, probs = self._buf("ic_logits", (M, V)), self._buf("ic_probs", (2, M, _pitch(V)))
+        layernorm(x, *self._packed["after_norm"], LN_EPS, out_plain=h, out_split=hs)
+        ctc.logits(h, hs, out=logits)
+        ops.softmax_rows_split(logits, probs)
+        linear(probs, self._packed["cond_w"], x, bias=self._packed["cond_b"], residual=x)
+        return h
 
     def _output(self, x, B, T):
         """after_norm into a new (B, T, D) tensor and its split copy (last_split_out) -> (out, out_split)."""

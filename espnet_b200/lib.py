@@ -62,6 +62,7 @@ _SIGS = {
     "espb_gather_rows_f32": [P, I, L, P, I, I, P, P],
     "espb_log_softmax_rows_f32": [P, L, L, I, P],
     "espb_argmax_rows_f32": [P, L, L, I, P, P],
+    "espb_softmax_rows_split_f32": [P, L, L, I, P, L, L, P],
     "espb_ctc_collapse_i32": [P, I, I, P, I, P, P, P],
     "espb_dec_embed_f32": [P, P, P, I, P, I, I, F, P, P],
     "espb_dec_self_attn_f32": [P, P, P, P, I, I, I, I, I, P, I, P, L, P],

@@ -139,6 +139,13 @@ def log_softmax_rows_(x2d):
     _count()
 
 
+def softmax_rows_split(x2d, out_split):
+    """out_split [2][rows][ldo] = tf32 hi / lo of the row softmax of x2d [rows][V]; columns V..ldo-1 zero (ldo % 32 == 0)."""
+    call("espb_softmax_rows_split_f32", ptr(x2d), x2d.shape[0], x2d.stride(0), x2d.shape[1], ptr(out_split), out_split[0].numel(),
+         out_split.shape[2])
+    _count()
+
+
 def argmax_rows(x2d, out):
     call("espb_argmax_rows_f32", ptr(x2d), x2d.shape[0], x2d.stride(0), x2d.shape[1], ptr(out))
     _count()

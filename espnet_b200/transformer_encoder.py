@@ -1,5 +1,5 @@
 """TransformerEncoder (absolute positions, conv2d / conv2d2 / conv2d6 / conv2d8 input layer, pre-LN, ReLU feed-forward) with the reference's constructor /
-state_dict surface -- the encoder of the next scope row (SURVEY.md 8f-1, BASELINE configs[4]).  It composes the kernels of the
+state_dict surface -- the encoder of the next scope row (SURVEY.md 8f-1, BASELINE configs[4]), with intermediate CTC and self-conditioning (interctc_layer_idx / interctc_use_conditioning).  It composes the kernels of the
 Conformer path (conv1 / implicit-GEMM conv2 / wgmma 3xTF32 GEMMs / LayerNorm) plus a plain masked softmax; the subsampling, FFN and
 self-attention are the shared ones of layers.py.
 
@@ -9,7 +9,7 @@ Parity: tests/test_gpu_zz_next.py (reference fixture layer by layer, ragged batc
 is the fused wgmma kernel without the rel-pos term (csrc/attention.cu) at d_k = 64.
 """
 import math
-from typing import List, Optional, Tuple
+from typing import List, Optional
 
 import torch
 
@@ -40,13 +40,14 @@ class TransformerEncoder(EncoderBase):
                  positionwise_conv_kernel_size: int = 1, padding_idx: int = -1, interctc_layer_idx: List[int] = [],
                  interctc_use_conditioning: bool = False, layer_drop_rate: float = 0.0, qk_norm: bool = False, use_flash_attn: bool = True):
         if (input_layer not in SUBSAMPLING or pos_enc_layer_type != "abs_pos" or not normalize_before or concat_after
-                or positionwise_layer_type != "linear" or qk_norm or len(interctc_layer_idx)):
-            raise NotImplementedError("espnet_b200 TransformerEncoder: conv2d / conv2d2 / conv2d6 / conv2d8 input, abs_pos, pre-LN, linear feed-forward, no interCTC / qk_norm")
+                or positionwise_layer_type != "linear" or qk_norm):
+            raise NotImplementedError("espnet_b200 TransformerEncoder: conv2d / conv2d2 / conv2d6 / conv2d8 input, abs_pos, pre-LN, linear feed-forward, no qk_norm")
         assert output_size % attention_heads == 0
         if output_size % 32:
             raise NotImplementedError("espnet_b200 TransformerEncoder: output_size must be a multiple of 32")
         super().__init__(input_size, output_size, (_Layer(output_size, linear_units) for _ in range(num_blocks)), input_layer)
         self.heads, self.num_blocks = attention_heads, num_blocks
+        self._init_interctc(interctc_layer_idx, interctc_use_conditioning, num_blocks)
         self._pe = {}
 
     def _pack(self):
@@ -57,9 +58,11 @@ class TransformerEncoder(EncoderBase):
         return pk
 
     @torch.no_grad()
-    def forward(self, xs_pad: torch.Tensor, ilens: torch.Tensor, prev_states: torch.Tensor = None
-                ) -> Tuple[torch.Tensor, torch.Tensor, Optional[torch.Tensor]]:
-        """xs_pad (B, T_f, idim) float32 CUDA, ilens (B,) -> (B, T, D), olens, None; per-utterance semantics for ragged batches."""
+    def forward(self, xs_pad: torch.Tensor, ilens: torch.Tensor, prev_states: torch.Tensor = None, ctc=None):
+        """xs_pad (B, T_f, idim) float32 CUDA, ilens (B,) -> (B, T, D), olens, None; per-utterance semantics for ragged batches.  With
+        interctc_layer_idx the first element is ((B, T, D), [(layer, intermediate output), ...]) and, with interctc_use_conditioning, ctc is
+        the CTC head (transformer_encoder.py:216-299)."""
+        self._check_interctc(ctc)
         pk = self._packed or self._pack()
         xs_pad, T, olens, lens32 = self._lengths(xs_pad, ilens)   # check_short_utt: transformer_encoder.py:253-262
         B, D = xs_pad.shape[0], self._output_size
@@ -76,7 +79,8 @@ class TransformerEncoder(EncoderBase):
             self.trace.append(x.view(B, T, D).clone())
         fused = ops.use_flash_attn(D // self.heads)   # one wgmma kernel for q k^T + masked softmax + p v (csrc/attention.cu)
         xn, qkv, ctx = self._buf("xn", (2, M, D)), self._buf("qkv", (2, M, 3 * D)), self._buf("ctx", (2, M, D))
-        for w in pk["layers"]:
+        inter = []
+        for li, w in enumerate(pk["layers"]):
             # x += MHA(LN1(x))  (encoder_layer.py:91-110, attention.py:262-265)
             layernorm(x, *w["n1"], LN_EPS, out_split=xn)
             linear(xn, w["qkv_w"], qkv, bias=w["qkv_b"], split_out=True)
@@ -86,5 +90,7 @@ class TransformerEncoder(EncoderBase):
             self._ffn(x, xn, w["n2"], w["ffn"], ACT_RELU, 1.0)
             if self.trace is not None:
                 self.trace.append(x.view(B, T, D).clone())
+            if li + 1 in self.interctc_layer_idx:
+                inter.append((li + 1, self._interctc(x, B, T, ctc)))
         out, _ = self._output(x, B, T)
-        return out, olens, None
+        return ((out, inter) if inter else out), olens, None

@@ -172,6 +172,11 @@ int espb_gather_rows_f32(const float* src, int N, long long src_rows, const int*
 /* ---- CTC head (espnet2/asr/ctc.py:197-215; greedy collapse asr_inference.py:574-575, s2t_inference_ctc.py:630-632) ---- */
 int espb_log_softmax_rows_f32(float* x, long long rows, long long ld, int V, cudaStream_t stream);
 int espb_argmax_rows_f32(const float* x, long long rows, long long ld, int V, int* out, cudaStream_t stream);
+/* Self-conditioned intermediate CTC: out / out + out_plane [rows][ldo] = tf32 hi / lo of softmax(x[r][0..V-1]) (x row pitch ld), columns
+ * V..ldo-1 written as zeros, so the result is the A operand of a 3xTF32 GEMM with K = ldo.  Refused with ESPB_ERR_ARG unless V > 0,
+ * ld >= V, ldo >= V with ldo % 32 == 0 and out_plane >= rows * ldo. */
+int espb_softmax_rows_split_f32(const float* x, long long rows, long long ld, int V, float* out, long long out_plane, long long ldo,
+                                cudaStream_t stream);
 int espb_ctc_collapse_i32(const int* argmax, int B, int Tmax, const int* lens, int blank, int* out_ids, int* out_len, cudaStream_t stream);
 
 /* ---- Decoder step (transformer_decoder.py:191-311, decoder_layer.py:73-179, embedding.py:38-95) -------------------------
