@@ -1,13 +1,8 @@
 // C-ABI surface shared bits: last-error string, version, GEMM entry point (see include/espnet_b200.h).
-#include <stdlib.h>
 #include <string.h>
 
 #include "common.cuh"
 #include "gemm.h"
-
-#ifndef ESPB_PDL_DEFAULT
-#define ESPB_PDL_DEFAULT 1
-#endif
 
 static thread_local char g_err[512] = "";
 
@@ -15,15 +10,6 @@ void espb_set_error(const char* msg) {
   strncpy(g_err, msg ? msg : "", sizeof(g_err) - 1);
   g_err[sizeof(g_err) - 1] = 0;
 }
-
-namespace espb {
-// ESPB_PDL=1 / 0 overrides the default; read once.
-bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("ESPB_PDL"); v = e ? (e[0] == '1') : ESPB_PDL_DEFAULT; }
-  return v == 1;
-}
-}  // namespace espb
 
 extern "C" {
 

@@ -25,10 +25,8 @@ constexpr int ACT_NONE = 0, ACT_RELU = 1, ACT_SWISH = 2, ACT_GELU = 3;
 // before its first global-memory access (setup that touches only shared memory / barriers may precede it).  pdl_trigger()
 // lets the next kernel in the stream do the same.  Every kernel of the chain waits before it completes, so completion order --
 // and with it every read-after-write / write-after-read dependency of plain stream order -- is preserved transitively.
-// ESPB_PDL=0 launches with full stream serialisation; griddepcontrol.* are no-ops then.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-bool pdl_enabled();
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args... args) {
   cudaLaunchConfig_t cfg = {};
@@ -37,7 +35,7 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 

@@ -2,8 +2,6 @@
 // self-conditioning GEMM of intermediate CTC.
 // Reference: espnet2/asr/ctc.py:187-215 (softmax, log_softmax, argmax), espnet2/asr/encoder/conformer_encoder.py:394-414 (conditioning),
 // espnet2/bin/asr_inference.py:574-575 and espnet2/bin/s2t_inference_ctc.py:630-632 (unique_consecutive + drop blank).
-#include <stdlib.h>
-
 #include "common.cuh"
 
 namespace {
@@ -163,11 +161,9 @@ extern "C" {
 
 int espb_log_softmax_rows_f32(float* x, long long rows, long long ld, int V, cudaStream_t stream) {
   if (rows <= 0) return ESPB_OK;
-  static int three_pass = -1;
-  if (three_pass < 0) three_pass = getenv("ESPB_LOGSOFTMAX_3PASS") ? 1 : 0;
-  if (!three_pass && V <= 256 * 8) espb::launch_pdl(log_softmax_rows_reg_kernel<8>, dim3((unsigned)rows), dim3(256), 0, stream, x, ld, V);
-  else if (!three_pass && V <= 256 * 20) espb::launch_pdl(log_softmax_rows_reg_kernel<20>, dim3((unsigned)rows), dim3(256), 0, stream, x, ld, V);
-  else if (!three_pass && V <= 256 * 32) espb::launch_pdl(log_softmax_rows_reg_kernel<32>, dim3((unsigned)rows), dim3(256), 0, stream, x, ld, V);
+  if (V <= 256 * 8) espb::launch_pdl(log_softmax_rows_reg_kernel<8>, dim3((unsigned)rows), dim3(256), 0, stream, x, ld, V);
+  else if (V <= 256 * 20) espb::launch_pdl(log_softmax_rows_reg_kernel<20>, dim3((unsigned)rows), dim3(256), 0, stream, x, ld, V);
+  else if (V <= 256 * 32) espb::launch_pdl(log_softmax_rows_reg_kernel<32>, dim3((unsigned)rows), dim3(256), 0, stream, x, ld, V);
   else espb::launch_pdl(log_softmax_rows_kernel, dim3((unsigned)rows), dim3(256), 0, stream, x, ld, V);
   ESPB_CHECK_LAUNCH();
   return ESPB_OK;

@@ -7,7 +7,6 @@
 // Reference: espnet2/legacy/nets/pytorch_backend/transformer/{layer_norm,subsampling,attention}.py,
 // .../conformer/{convolution,encoder_layer}.py (line ranges at each kernel).
 #include <stdint.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 
@@ -773,7 +772,7 @@ int espb_layernorm_f32(const float* x, long long rows, int D, const float* gamma
   {
     const uintptr_t al = reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(beta) |
                          reinterpret_cast<uintptr_t>(out_plain) | reinterpret_cast<uintptr_t>(out_split);
-    if ((D & 3) == 0 && D <= 1024 && (al & 15) == 0 && (split_plane & 3) == 0 && !getenv("ESPB_LN_SCALAR")) {
+    if ((D & 3) == 0 && D <= 1024 && (al & 15) == 0 && (split_plane & 3) == 0) {
       const int rpb = rows <= 4096 ? 2 : 8;   // rows (warps) per block
       const dim3 g((unsigned)((rows + rpb - 1) / rpb)), blk(32 * rpb);
       if (D <= 256) espb::launch_pdl(layernorm_vec_kernel<2>, g, blk, 0, stream, x, rows, D, gamma, beta, eps, out_plain, out_split, split_plane);
@@ -852,7 +851,7 @@ int espb_relpos_softmax_f32(const float* ac, const float* bd, int B, int H, int 
   // (a register-resident single-pass variant <NV> has lower occupancy; kept for short rows)
   if (T <= 128) relpos_softmax_kernel<4><<<grid, 256, 0, stream>>>(ac, bd, B, H, T, Tp, Rp, lens, sqrt_dk, probs, probs_plane);
   else if ((Tp & 3) == 0 && (probs_plane & 3) == 0 && (reinterpret_cast<uintptr_t>(ac) & 15) == 0 && (reinterpret_cast<uintptr_t>(probs) & 15) == 0 &&
-           (size_t)8 * Tp * sizeof(float) <= 48 * 1024 && !getenv("ESPB_SOFTMAX_3PASS"))
+           (size_t)8 * Tp * sizeof(float) <= 48 * 1024)
     relpos_softmax_smem_kernel<<<grid, 256, (size_t)8 * Tp * sizeof(float), stream>>>(ac, bd, B, H, T, Tp, Rp, lens, sqrt_dk, probs, probs_plane);
   else relpos_softmax_kernel<0><<<grid, 256, 0, stream>>>(ac, bd, B, H, T, Tp, Rp, lens, sqrt_dk, probs, probs_plane);
   ESPB_CHECK_LAUNCH();
@@ -871,12 +870,10 @@ int espb_glu_dwconv_bn_swish_f32(const float* y, int B, int Tmax, int C, const i
                                  const float* bn_a, const float* bn_b, float* out, long long out_plane, cudaStream_t stream) {
   if (K < 1 || (K & 1) == 0 || K > 127) { espb_set_error("dwconv: kernel size must be odd and <= 127"); return ESPB_ERR_ARG; }
   dim3 grid((Tmax + DW_TT - 1) / DW_TT, (C + DW_CC - 1) / DW_CC, B);
-  static int v1 = -1;
-  if (v1 < 0) v1 = getenv("ESPB_DWCONV_V1") ? 1 : 0;
   const size_t smem_win = (size_t)(DW_TT + K - 1) * DW_CC * sizeof(float);
-  if (!v1 && K == 31) {
+  if (K == 31) {
     glu_dwconv_bn_swish_win_kernel<31><<<grid, 256, smem_win, stream>>>(y, Tmax, C, lens, dw_w, dw_b, bn_a, bn_b, out, out_plane);
-  } else if (!v1 && K == 15) {
+  } else if (K == 15) {
     glu_dwconv_bn_swish_win_kernel<15><<<grid, 256, smem_win, stream>>>(y, Tmax, C, lens, dw_w, dw_b, bn_a, bn_b, out, out_plane);
   } else {
     // tile + weights: 49 408 B at K = 65, 81 152 B at K = 127 -- past the 48 KB a launch gets without opting in

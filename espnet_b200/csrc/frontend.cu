@@ -5,15 +5,12 @@
 // Reference: espnet2/layers/stft.py:75-120, espnet2/asr/frontend/default.py:82-117,
 // espnet2/layers/log_mel.py:57-84, espnet2/layers/utterance_mvn.py:45-88.
 #include <stdint.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 
 namespace {
 
-constexpr int NFFT = 512, HOP = 128, NC = 256;  // NC: complex points of the packed FFT
-constexpr int WARPS = 4, FRAMES_PER_WARP = 8, FRAMES_PER_BLOCK = WARPS * FRAMES_PER_WARP;
-constexpr int SEG = (FRAMES_PER_BLOCK - 1) * HOP + NFFT;  // samples a block touches (with overlap)
+constexpr int NFFT = 512, NC = 256;  // NC: complex points of the packed FFT
 
 struct MelSparse {          // filter m covers bins [start[m], start[m]+count[m]); weights packed at offset[m]
   const int* start; const int* count; const int* offset; const float* weight; int n_mels;
@@ -23,124 +20,6 @@ __device__ __forceinline__ int reflect_idx(int i, int L) {  // torch "reflect": 
   if (i < 0) i = -i;
   if (i >= L) i = 2 * (L - 1) - i;
   return i;
-}
-
-// One warp transforms one frame: z[n] = x[2n] + i x[2n+1] (windowed), 256-point radix-4 Stockham
-// FFT in shared memory, then the real-FFT split to get bins 0..256.
-__global__ void __launch_bounds__(WARPS * 32)
-stft_logmel_kernel(const float* __restrict__ wave, const long long* __restrict__ wave_lens, int Lmax, int B,
-                   const float* __restrict__ window, const float2* __restrict__ tw512, MelSparse mel,
-                   float* __restrict__ out, int Tf_max, float* __restrict__ partial /* [B][nblk][n_mels] */) {
-  __shared__ float seg[SEG];
-  __shared__ float win[NFFT];
-  __shared__ float2 tw[NC];             // exp(-2 pi i k / 512), k = 0..255
-  __shared__ float2 bufA[WARPS][NC];
-  __shared__ float2 bufB[WARPS][NC];
-  __shared__ float colsum[WARPS][96];
-
-  const int b = blockIdx.y, blk = blockIdx.x;
-  const int L = (int)wave_lens[b];
-  const int Tf = 1 + L / HOP;
-  const int f0 = blk * FRAMES_PER_BLOCK;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const float* w = wave + (long long)b * Lmax;
-
-  for (int i = threadIdx.x; i < NFFT; i += blockDim.x) win[i] = window[i];
-  for (int i = threadIdx.x; i < NC; i += blockDim.x) tw[i] = tw512[i];
-  const int s0 = f0 * HOP - NFFT / 2;   // first (un-reflected) sample index of this block's segment
-  if (L > 1) {
-    for (int i = threadIdx.x; i < SEG; i += blockDim.x) {
-      int g = s0 + i;
-      float v = 0.f;
-      if (g < L + NFFT / 2 && g > -NFFT) v = __ldg(w + reflect_idx(g, L));
-      seg[i] = v;
-    }
-  } else {
-    for (int i = threadIdx.x; i < SEG; i += blockDim.x) seg[i] = 0.f;
-  }
-  for (int i = lane; i < 96; i += 32) colsum[warp][i] = 0.f;
-  __syncthreads();
-
-  float2* A = bufA[warp];
-  float2* Bf = bufB[warp];
-  for (int fi = 0; fi < FRAMES_PER_WARP; ++fi) {
-    const int f = f0 + warp * FRAMES_PER_WARP + fi;
-    if (f >= Tf_max) break;                       // warp-uniform
-    float* orow = out + ((long long)b * Tf_max + f) * mel.n_mels;
-    if (f >= Tf) {                                // padded frame of a shorter utterance: zeros (stft.py:117, log_mel.py:78-81)
-      for (int m = lane; m < mel.n_mels; m += 32) orow[m] = 0.f;
-      continue;
-    }
-    const float* x = seg + (f - f0) * HOP;
-    // load + window + pack
-    for (int n = lane; n < NC; n += 32) A[n] = make_float2(x[2 * n] * win[2 * n], x[2 * n + 1] * win[2 * n + 1]);
-    __syncwarp();
-    // 4 radix-4 Stockham stages: N=256, Ns = 1,4,16,64
-    float2* src = A; float2* dst = Bf;
-#pragma unroll
-    for (int st = 0; st < 4; ++st) {
-      const int Ns = 1 << (2 * st);
-      for (int j = lane; j < NC / 4; j += 32) {
-        const int k = j & (Ns - 1);               // position within the current sub-transform
-        float2 v0 = src[j], v1 = src[j + 64], v2 = src[j + 128], v3 = src[j + 192];
-        // twiddle: exp(-2 pi i k r / (4 Ns)) = tw512[k r * 512/(4 Ns)]
-        const int tstep = (NFFT / (4 * Ns)) * k;  // index into tw512 for r=1
-        if (st > 0) {
-          // indices reach up to 3*tstep < 384: fold via tw512[i+256] = -tw512[i]
-          const int i2 = 2 * tstep, i3 = 3 * tstep;
-          float2 t1 = tw[tstep], t2, t3;
-          t2 = tw[i2 & 255]; if (i2 & 256) { t2.x = -t2.x; t2.y = -t2.y; }
-          t3 = tw[i3 & 255]; if (i3 & 256) { t3.x = -t3.x; t3.y = -t3.y; }
-          float2 u;
-          u = v1; v1.x = u.x * t1.x - u.y * t1.y; v1.y = u.x * t1.y + u.y * t1.x;
-          u = v2; v2.x = u.x * t2.x - u.y * t2.y; v2.y = u.x * t2.y + u.y * t2.x;
-          u = v3; v3.x = u.x * t3.x - u.y * t3.y; v3.y = u.x * t3.y + u.y * t3.x;
-        }
-        // radix-4 butterfly (forward: multiply by -i for the odd differences)
-        float2 a0 = make_float2(v0.x + v2.x, v0.y + v2.y), a1 = make_float2(v0.x - v2.x, v0.y - v2.y);
-        float2 a2 = make_float2(v1.x + v3.x, v1.y + v3.y), a3 = make_float2(v1.x - v3.x, v1.y - v3.y);
-        const int o = (j - k) * 4 + k;            // expand: block base * 4 + k
-        dst[o] = make_float2(a0.x + a2.x, a0.y + a2.y);
-        dst[o + Ns] = make_float2(a1.x + a3.y, a1.y - a3.x);
-        dst[o + 2 * Ns] = make_float2(a0.x - a2.x, a0.y - a2.y);
-        dst[o + 3 * Ns] = make_float2(a1.x - a3.y, a1.y + a3.x);
-      }
-      __syncwarp();
-      float2* t = src; src = dst; dst = t;
-    }
-    // src now holds Z[0..255]. Real split: X[k] = (Z[k]+conj(Z[N-k]))/2 - i/2 * w^k * (Z[k]-conj(Z[N-k]))
-    float* P = reinterpret_cast<float*>(dst);  // 4 swaps: src == bufA again, bufB is free for the power spectrum
-    for (int k = lane; k <= NC; k += 32) {
-      float2 zk = src[k & 255], zn = src[(NC - k) & 255];
-      float2 e = make_float2(0.5f * (zk.x + zn.x), 0.5f * (zk.y - zn.y));
-      float2 o = make_float2(0.5f * (zk.x - zn.x), 0.5f * (zk.y + zn.y));   // (Z[k]-conj(Z[N-k]))/2
-      float2 t = (k == NC) ? make_float2(-1.f, 0.f) : tw[k];
-      // -i * t * o
-      float2 to = make_float2(t.x * o.x - t.y * o.y, t.x * o.y + t.y * o.x);
-      float re = e.x + to.y, im = e.y - to.x;
-      P[k] = re * re + im * im;
-    }
-    __syncwarp();
-    for (int m = lane; m < mel.n_mels; m += 32) {
-      const int st0 = mel.start[m], cnt = mel.count[m];
-      const float* wm = mel.weight + mel.offset[m];
-      float acc = 0.f;
-      for (int i = 0; i < cnt; ++i) acc = fmaf(P[st0 + i], __ldg(wm + i), acc);
-      float v = logf(fmaxf(acc, 1e-10f));
-      orow[m] = v;
-      colsum[warp][m] += v;
-    }
-    __syncwarp();
-  }
-  __syncthreads();
-  if (partial) {
-    for (int m = threadIdx.x; m < mel.n_mels; m += blockDim.x) {
-      float s = 0.f;
-#pragma unroll
-      for (int wv = 0; wv < WARPS; ++wv) s += colsum[wv][m];
-      partial[((long long)b * gridDim.x + blk) * mel.n_mels + m] = s;
-    }
-  }
 }
 
 // ---------------------------------------------------------------- register-resident FFT (v2)
@@ -318,7 +197,7 @@ __global__ void utt_mvn_kernel(float* __restrict__ feats, const long long* __res
   }
 }
 
-// Column sums over valid frames for features that did not come from stft_logmel_kernel (standalone normalize).
+// Column sums over valid frames for features that did not come from stft_logmel_v2_kernel (standalone normalize).
 __global__ void feat_colsum_kernel(const float* __restrict__ feats, const long long* __restrict__ feat_lens, int Tf_max, int n_mels,
                                    float* __restrict__ partial, int nblk) {
   const int b = blockIdx.y, blk = blockIdx.x;
@@ -368,7 +247,7 @@ __global__ void global_mvn_kernel(float* __restrict__ feats, const long long* __
 
 extern "C" {
 
-int espb_frontend_blocks(int Tf_max) { return (Tf_max + FRAMES_PER_BLOCK - 1) / FRAMES_PER_BLOCK; }
+int espb_frontend_blocks(int Tf_max) { return (Tf_max + V2_FPB - 1) / V2_FPB; }
 
 int espb_stft_logmel_f32(const float* wave, const long long* wave_lens, int B, int Lmax, int hop, const float* window,
                          const float* tw512, const float* tw256t, const int* mel_start, const int* mel_count, const int* mel_offset,
@@ -378,12 +257,6 @@ int espb_stft_logmel_f32(const float* wave, const long long* wave_lens, int B, i
   }
   MelSparse mel{mel_start, mel_count, mel_offset, mel_weight, n_mels};
   dim3 grid(espb_frontend_blocks(Tf_max), B);
-  if (hop == HOP && n_mels <= 96 && getenv("ESPB_STFT_V1")) {   // round-1 kernel (shared-memory radix-4 FFT), kept for A/B measurements
-    stft_logmel_kernel<<<grid, WARPS * 32, 0, stream>>>(wave, wave_lens, Lmax, B, window, reinterpret_cast<const float2*>(tw512),
-                                                        mel, out, Tf_max, partial);
-    ESPB_CHECK_LAUNCH();
-    return ESPB_OK;
-  }
   const int seg_n = (V2_FPB - 1) * hop + NFFT;
   const size_t smem = ((size_t)((seg_n + 3) & ~3) + NFFT + 2 * NC * 2 + (size_t)V2_WARPS * 2 * 16 * 17 * 2 + ((mel_nnz + 3) & ~3) + 3 * n_mels +
                        (size_t)V2_WARPS * 2 * n_mels) * sizeof(float);

@@ -7,8 +7,6 @@
 // beam_search.py:385-498 (loop, maxlen/minlen), e2e_asr_common.py:14-44 (end_detect),
 // ctc_prefix_score.py:71-191 + scorers/ctc.py:40-63,101-126 (CTC prefix scorer),
 // asr/decoder/transformer_decoder.py:191-311 + transformer/decoder_layer.py:73-179 (decoder step).
-#include <stdlib.h>
-
 #include "common.cuh"
 
 namespace {
@@ -212,20 +210,15 @@ __global__ void __launch_bounds__(128) dec_self_attn64_kernel(const float* __res
 // q [n][D]; memory K / V blocks are contiguous per (utterance, head): kmem/vmem + ((u*H + h)*Tmax + t)*dk + d  (written once per
 // utterance by the K/V projection GEMMs and shared by the whole beam).  One block per (utterance, head): the K and V blocks are
 // streamed exactly once with coalesced 128-bit loads (LPR lanes per row, several rows per warp instruction, UN instructions in flight).
-// WC / DKC: compile-time beam size / head dim (0 = run-time values): the specialised instances have no predicates in the inner loops.
-template <int UN, int WC, int DKC>
+template <int UN>
 __global__ void __launch_bounds__(256, 3) dec_src_attn_kernel(const float* __restrict__ q, const float* __restrict__ kmem, const float* __restrict__ vmem,
-                                                           int Tmax, const int* __restrict__ lens, int W_rt, int D, int H, int lpr_rt /* pow2 >= dk/4 */,
+                                                           int Tmax, const int* __restrict__ lens, int W, int D, int H, int lpr /* pow2 >= dk/4 */,
                                                            float* __restrict__ ctx, long long ctx_plane, int w0, int Wall) {
   extern __shared__ float sm[];  // q [W][dk] | scores [W][Tmax] (reused for the cross-warp PV reduction) | K tile [128][dk+4]
   espb::pdl_trigger();
   espb::pdl_wait();
-  constexpr bool CT = (WC > 0);
-  constexpr int JMAX = CT ? (WC + 1) / 2 : 8;          // beam slots per half block
-  constexpr bool FULL = CT && (WC % 2 == 0);           // both halves own exactly JMAX slots
-  const int W = CT ? WC : W_rt;
-  const int dk = (DKC > 0) ? DKC : D / H;
-  const int lpr = (DKC == 64) ? 16 : lpr_rt;
+  constexpr int JMAX = 8;          // beam slots per half block
+  const int dk = D / H;
   const int u = blockIdx.x / H, h = blockIdx.x % H;
   const int T = lens[u];
   float* qs = sm;
@@ -263,14 +256,14 @@ __global__ void __launch_bounds__(256, 3) dec_src_attn_kernel(const float* __res
 #pragma unroll
           for (int j = 0; j < JMAX; ++j) {
             const int w = w_lo + j;
-            if (FULL || w < w_hi) {
+            if (w < w_hi) {
               const float4 q4 = *reinterpret_cast<const float4*>(qs + w * dk + d0);
               a[j] = fmaf(q4.x, k4.x, a[j]); a[j] = fmaf(q4.y, k4.y, a[j]); a[j] = fmaf(q4.z, k4.z, a[j]); a[j] = fmaf(q4.w, k4.w, a[j]);
             }
           }
         }
 #pragma unroll
-        for (int j = 0; j < JMAX; ++j) if (FULL || w_lo + j < w_hi) sc[(w_lo + j) * Tmax + tb + r] = a[j] / rs;
+        for (int j = 0; j < JMAX; ++j) if (w_lo + j < w_hi) sc[(w_lo + j) * Tmax + tb + r] = a[j] / rs;
       }
       __syncthreads();
     }
@@ -307,7 +300,7 @@ __global__ void __launch_bounds__(256, 3) dec_src_attn_kernel(const float* __res
       const int t = min(t0 + uu * rpw + rsub, T - 1);   // rows beyond T carry v = 0
 #pragma unroll
       for (int j = 0; j < JMAX; ++j) {
-        if (FULL || w_lo + j < w_hi) {
+        if (w_lo + j < w_hi) {
           const float pw = sc[(w_lo + j) * Tmax + t];
           acc[j].x = fmaf(pw, vv[uu].x, acc[j].x); acc[j].y = fmaf(pw, vv[uu].y, acc[j].y);
           acc[j].z = fmaf(pw, vv[uu].z, acc[j].z); acc[j].w = fmaf(pw, vv[uu].w, acc[j].w);
@@ -318,7 +311,7 @@ __global__ void __launch_bounds__(256, 3) dec_src_attn_kernel(const float* __res
   // reduce over the rpw row groups of the warp (lanes with equal c4), then across the warps of the half through smem
 #pragma unroll
   for (int j = 0; j < JMAX; ++j) {
-    if (FULL || w_lo + j < w_hi) {
+    if (w_lo + j < w_hi) {
       for (int o = lpr; o < 32; o <<= 1) {
         acc[j].x += __shfl_xor_sync(0xffffffffu, acc[j].x, o); acc[j].y += __shfl_xor_sync(0xffffffffu, acc[j].y, o);
         acc[j].z += __shfl_xor_sync(0xffffffffu, acc[j].z, o); acc[j].w += __shfl_xor_sync(0xffffffffu, acc[j].w, o);
@@ -330,7 +323,7 @@ __global__ void __launch_bounds__(256, 3) dec_src_attn_kernel(const float* __res
   if (rsub == 0 && col_ok) {
 #pragma unroll
     for (int j = 0; j < JMAX; ++j)
-      if (FULL || w_lo + j < w_hi) *reinterpret_cast<float4*>(red + ((long long)wh * W + w_lo + j) * dk + c4 * 4) = acc[j];
+      if (w_lo + j < w_hi) *reinterpret_cast<float4*>(red + ((long long)wh * W + w_lo + j) * dk + c4 * 4) = acc[j];
   }
   __syncthreads();
   for (int i = threadIdx.x; i < W * dk; i += blockDim.x) {
@@ -340,10 +333,9 @@ __global__ void __launch_bounds__(256, 3) dec_src_attn_kernel(const float* __res
   }
 }
 
-// ---------------------------------------------------------------- cross-attention on the tensor cores (d_k = 64, beam <= 16)
-// Same contract as dec_src_attn_kernel.  Scores S[t][slot] = K_tile[t][:] . Q[slot][:] and the context O[slot][d] = sum_t P[slot][t] V[t][d] are
-// m16n8k8 TF32 mma.sync products with the 3xTF32 error compensation (operands split into hi/lo in registers), fed from smem-staged K / V
-// tiles; this removes ~4/5 of the FFMA/LDS instructions that bound the CUDA-core version (ncu: 99 M warp instructions, 46 % issue-active).
+// ---------------------------------------------------------------- tensor-core helpers of the cross-attention (d_k = 64, beam <= 16)
+// m16n8k8 TF32 mma.sync products with the 3xTF32 error compensation (operands split into hi/lo in registers), and the cp.async copies that
+// stage the K / V tiles in shared memory.
 __device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
   hi = __float_as_uint(x) & 0xFFFFE000u;
   lo = __float_as_uint(x - __uint_as_float(hi)) & 0xFFFFE000u;
@@ -367,177 +359,20 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-// The K tiles and then the V tiles of one (utterance, head) stream through an S-deep cp.async ring of 64-frame tiles (one
-// __syncthreads per tile; S-1 tiles in flight per block, two blocks per SM), so the HBM read of the encoder memory -- the
-// algorithmic cost of this kernel -- is never stalled behind the mma phases; the softmax runs while the first V tiles land.
-template <int S>
-__global__ void __launch_bounds__(256, 2) dec_src_attn_mma_kernel(const float* __restrict__ q, const float* __restrict__ kmem, const float* __restrict__ vmem,
-                                                                  int Tmax, const int* __restrict__ lens, int W, int D, int H,
-                                                                  float* __restrict__ ctx, long long ctx_plane, int w0, int Wall) {
-  constexpr int DK = 64, QST = 68, KST = 68, VST = 72, TR = 64, TILE_F = TR * VST;
-  extern __shared__ float sm[];  // q [16][68] | scores [W][Tmax] (pad 4) | ring [S][64][72] (reused for the cross-warp reduction)
-  espb::pdl_trigger();
-  espb::pdl_wait();
-  const int u = blockIdx.x / H, h = blockIdx.x % H;
-  const int T = lens[u];
-  float* qs = sm;
-  float* sc = qs + 16 * QST;
-  float* ring = sc + (((long long)W * Tmax + 3) & ~3LL);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int g = lane >> 2, t4 = lane & 3;
-  const float4* kb = reinterpret_cast<const float4*>(kmem + ((long long)(u * H + h) * Tmax) * DK);
-  const float4* vb = reinterpret_cast<const float4*>(vmem + ((long long)(u * H + h) * Tmax) * DK);
-  const int nt = (T + TR - 1) / TR, NT = 2 * nt;
-  auto issue = [&](int i) {
-    if (i < NT) {
-      const bool isk = i < nt;
-      const int tb = (isk ? i : i - nt) * TR;
-      const float4* src = isk ? kb : vb;
-      const int st = isk ? KST : VST;
-      float* dst = ring + (i % S) * TILE_F;
-#pragma unroll
-      for (int j = threadIdx.x; j < TR * 16; j += 256) {
-        const int rr = j >> 4, cc = j & 15;
-        const bool ok = tb + rr < T;      // frames past the utterance are zero-filled (src-size 0)
-        cp_async16_zfill(dst + rr * st + cc * 4, src + (ok ? (long long)(tb + rr) * 16 + cc : 0), ok ? 16 : 0);
-      }
-    }
-    cp_async_commit();                    // one (possibly empty) group per tile index keeps the wait_group arithmetic uniform
-  };
-#pragma unroll
-  for (int i = 0; i < S - 1; ++i) issue(i);
-  for (int i = threadIdx.x; i < 16 * DK; i += blockDim.x) {
-    const int w = i / DK, d = i % DK;
-    qs[w * QST + d] = (w < W) ? q[((long long)(u * Wall + w0 + w)) * D + h * DK + d] : 0.f;
-  }
-  const float rs = 8.0f;   // sqrt(d_k)
-  const int sa = min(g, W - 1), sb = min(g + 8, W - 1);
-  __syncthreads();         // qs is complete
-
-  // ================================================================= K phase: S[slot][t] = Q[slot][:] . K[t][:]
-  // A = Q (16 slot rows x 8 d per k-step, the same for every tile: split once into registers), B = K^T (8 d x 8 frames): warp w owns
-  // frames 8w..8w+7 of each 64-frame tile, so every K element is read from smem and split exactly once (the earlier layout -- A = K rows,
-  // B = Q^T -- split every K element in two warps and re-split Q for every tile: 3x the instructions of this loop; the kernel is
-  // issue-bound, not HBM-bound: ncu r01 30 % tensor pipe, 2.9 TB/s).
-  {
-    uint32_t qh[8][4], ql[8][4];
-#pragma unroll
-    for (int ks = 0; ks < 8; ++ks) {
-      split_tf32(qs[g * QST + ks * 8 + t4], qh[ks][0], ql[ks][0]);
-      split_tf32(qs[(g + 8) * QST + ks * 8 + t4], qh[ks][1], ql[ks][1]);
-      split_tf32(qs[g * QST + ks * 8 + t4 + 4], qh[ks][2], ql[ks][2]);
-      split_tf32(qs[(g + 8) * QST + ks * 8 + t4 + 4], qh[ks][3], ql[ks][3]);
-    }
-    for (int i = 0; i < nt; ++i) {
-      cp_async_wait<S - 2>();               // this thread's copies of tile i have landed ...
-      __syncthreads();                      // ... and everyone's; all warps are done with tile i-1, whose slot is refilled next
-      issue(i + S - 1);
-      const float* tile = ring + (i % S) * TILE_F;
-      const int tb = i * TR, rows = min(TR, T - tb);
-      const int f0 = warp * 8;
-      if (f0 < rows) {
-        // one accumulator per product term: three independent 8-deep mma chains instead of one 24-deep chain
-        float c[4] = {0.f, 0.f, 0.f, 0.f}, c1[4] = {0.f, 0.f, 0.f, 0.f}, c2[4] = {0.f, 0.f, 0.f, 0.f};
-        const float* kr = tile + (f0 + g) * KST + t4;
-#pragma unroll
-        for (int ks = 0; ks < 8; ++ks) {
-          uint32_t bh[2], bl[2];
-          split_tf32(kr[ks * 8], bh[0], bl[0]);
-          split_tf32(kr[ks * 8 + 4], bh[1], bl[1]);
-          mma_m16n8k8_tf32(c1, ql[ks], bh);
-          mma_m16n8k8_tf32(c2, qh[ks], bl);
-          mma_m16n8k8_tf32(c, qh[ks], bh);
-        }
-#pragma unroll
-        for (int e = 0; e < 4; ++e) c[e] += c1[e] + c2[e];   // small terms combined first
-        const int fa = tb + f0 + 2 * t4;                      // C fragment: rows (slots) g, g+8; columns (frames) 2*t4, 2*t4+1
-        if (g < W) { if (fa < T) sc[g * Tmax + fa] = c[0] / rs; if (fa + 1 < T) sc[g * Tmax + fa + 1] = c[1] / rs; }
-        if (g + 8 < W) { if (fa < T) sc[(g + 8) * Tmax + fa] = c[2] / rs; if (fa + 1 < T) sc[(g + 8) * Tmax + fa + 1] = c[3] / rs; }
-      }
-    }
-  }
-
-  // ================================================================= V phase: O[slot][d] = sum_t P[slot][t] V[t][d]
-  float acc[8][4];
-#pragma unroll
-  for (int n8 = 0; n8 < 8; ++n8) { acc[n8][0] = 0.f; acc[n8][1] = 0.f; acc[n8][2] = 0.f; acc[n8][3] = 0.f; }
-  for (int i = nt; i < NT; ++i) {
-    cp_async_wait<S - 2>();
-    __syncthreads();
-    issue(i + S - 1);
-    if (i == nt) {
-      // ---- softmax over t per slot (no memory mask: batch_score passes none, transformer_decoder.py:294-303); the first V tiles land meanwhile
-      for (int w = warp; w < W; w += 8) {
-        float* r = sc + w * Tmax;
-        float mx = -INFINITY;
-        for (int t = lane; t < T; t += 32) mx = fmaxf(mx, r[t]);
-        mx = espb::warp_max(mx);
-        float sum = 0.f;
-        for (int t = lane; t < T; t += 32) { float e = expf(r[t] - mx); r[t] = e; sum += e; }
-        sum = espb::warp_sum(sum);
-        for (int t = lane; t < T; t += 32) r[t] = r[t] / sum;
-      }
-      __syncthreads();
-    }
-    const float* tile = ring + (i % S) * TILE_F;
-    {
-      // ---- context: A = P (16 slot rows, clamped to W-1), B = V tile, K-dim = t (warp w takes the 8-frame k-step w of the tile)
-      const int tb = (i - nt) * TR, rows = min(TR, T - tb);
-      if (warp * 8 < rows) {
-        const int t0 = tb + warp * 8 + t4, t1 = t0 + 4;
-        uint32_t ah[4], al[4];
-        split_tf32(t0 < T ? sc[sa * Tmax + t0] : 0.f, ah[0], al[0]);
-        split_tf32(t0 < T ? sc[sb * Tmax + t0] : 0.f, ah[1], al[1]);
-        split_tf32(t1 < T ? sc[sa * Tmax + t1] : 0.f, ah[2], al[2]);
-        split_tf32(t1 < T ? sc[sb * Tmax + t1] : 0.f, ah[3], al[3]);
-#pragma unroll
-        for (int n8 = 0; n8 < 8; ++n8) {
-          uint32_t bh[2], bl[2];
-          split_tf32(tile[(warp * 8 + t4) * VST + n8 * 8 + g], bh[0], bl[0]);
-          split_tf32(tile[(warp * 8 + t4 + 4) * VST + n8 * 8 + g], bh[1], bl[1]);
-          mma3_tf32(acc[n8], ah, al, bh, bl);
-        }
-      }
-    }
-  }
-  cp_async_wait<0>();
-  __syncthreads();
-  // ---- cross-warp reduction: red[warp][slot 16][d 64] (32 KB) in the ring, then split store of the W valid slots
-  float* red = ring;
-  static_assert(S * TILE_F >= 8 * 16 * DK, "reduction scratch must fit in the ring");
-#pragma unroll
-  for (int n8 = 0; n8 < 8; ++n8) {
-    float* r0p = red + ((long long)warp * 16 + g) * DK + n8 * 8 + 2 * t4;
-    float* r1p = red + ((long long)warp * 16 + g + 8) * DK + n8 * 8 + 2 * t4;
-    r0p[0] = acc[n8][0]; r0p[1] = acc[n8][1];
-    r1p[0] = acc[n8][2]; r1p[1] = acc[n8][3];
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < W * DK; i += blockDim.x) {
-    const int w = i / DK, d = i % DK;
-    float a = 0.f;
-#pragma unroll
-    for (int ww = 0; ww < 8; ++ww) a += red[((long long)ww * 16 + w) * DK + d];
-    store_split(ctx + ((long long)(u * Wall + w0 + w)) * D + h * DK + d, ctx_plane, a);
-  }
-}
-
-#ifndef ESPB_SRC_ATTN_NW_DEFAULT
-#define ESPB_SRC_ATTN_NW_DEFAULT 4
-#endif
 // ---------------------------------------------------------------- cross-attention, single pass (d_k = 64, beam <= 16, any T)
-// Flash-decoding inside a block: K and V tiles of 64 frames stream TOGETHER through an S-deep cp.async ring (no [W][T] score buffer, so twice
-// the bytes are in flight per SM and T is unbounded); warp w owns frames 8w..8w+7 of every tile and keeps its own online-softmax state
-// (running max / partial sum per slot, partial context [16][64] in mma accumulators); the eight partial results are merged once at the end.
+// Flash-decoding inside a block: K and V tiles of 8 FLASH_NW frames stream together through an S-deep cp.async ring (no [W][T] score buffer,
+// so T is unbounded); warp w owns frames 8w..8w+7 of every tile and keeps its own online-softmax state (running max / partial sum per
+// slot, partial context [16][64] in mma accumulators); the FLASH_NW partial results are merged once at the end.
 //   scores  C[16 slots][8 frames] = Q (A, split once into registers / smem) x K^T (B): every K element is read and split once
 //   context O[16 slots][64]      += P (A = the C fragment re-used in place: the k index of the second product is simply a permutation of
 //                                   the warp's 8 frames, lane t4 holds frames 2 t4, 2 t4 + 1) x V (B rows picked with the same permutation)
-template <int S, int NW>   // NW warps per block, 8 NW frames per tile: NW = 4 -> four 57 KB blocks per SM, all U x H blocks of a 64 x 8 launch resident at once
-__global__ void __launch_bounds__(NW * 32, 16 / NW) dec_src_attn_flash_kernel(const float* __restrict__ q, const float* __restrict__ kmem, const float* __restrict__ vmem,
+constexpr int FLASH_NW = 4;   // warps per block: four 57 KB blocks per SM, all U x H blocks of a 64 x 8 launch resident at once
+template <int S>
+__global__ void __launch_bounds__(FLASH_NW * 32, 16 / FLASH_NW) dec_src_attn_flash_kernel(const float* __restrict__ q, const float* __restrict__ kmem, const float* __restrict__ vmem,
                                                                     int Tmax, const int* __restrict__ lens, int W, int D, int H,
                                                                     float* __restrict__ ctx, long long ctx_plane, int w0, int Wall) {
-  constexpr int DK = 64, QST = 68, ST = 68, TR = 8 * NW, TILE_F = TR * ST, STAGE_F = 2 * TILE_F;
-  extern __shared__ float sm[];  // q lo [16][68] | ring [S][K [64][68] | V [64][68]] (reused for the cross-warp merge)
+  constexpr int DK = 64, QST = 68, ST = 68, TR = 8 * FLASH_NW, TILE_F = TR * ST, STAGE_F = 2 * TILE_F;
+  extern __shared__ float sm[];  // q lo [16][68] | ring [S][K [TR][68] | V [TR][68]] (reused for the cross-warp merge)
   espb::pdl_trigger();
   espb::pdl_wait();
   const int u = blockIdx.x / H, h = blockIdx.x % H;
@@ -554,7 +389,7 @@ __global__ void __launch_bounds__(NW * 32, 16 / NW) dec_src_attn_flash_kernel(co
       const int tb = i * TR;
       float* dst = ring + (i % S) * STAGE_F;
 #pragma unroll
-      for (int j = threadIdx.x; j < 2 * TR * 16; j += NW * 32) {
+      for (int j = threadIdx.x; j < 2 * TR * 16; j += FLASH_NW * 32) {
         const int isv = j / (TR * 16), rr = (j >> 4) % TR, cc = j & 15;
         const bool ok = tb + rr < T;      // frames past the utterance are zero-filled (src-size 0)
         cp_async16_zfill(dst + isv * TILE_F + rr * ST + cc * 4, (isv ? vb : kb) + (ok ? (long long)(tb + rr) * 16 + cc : 0), ok ? 16 : 0);
@@ -564,7 +399,7 @@ __global__ void __launch_bounds__(NW * 32, 16 / NW) dec_src_attn_flash_kernel(co
   };
 #pragma unroll
   for (int i = 0; i < S - 1; ++i) issue(i);
-  // Q A-fragments: hi parts in registers, lo parts in shared memory (register budget: 128 per thread at two blocks per SM)
+  // Q A-fragments: hi parts in registers, lo parts in shared memory (register budget: 128 per thread at four blocks per SM)
   uint32_t qh[8][4];
   {
     const float* qg = q + ((long long)(u * Wall + w0)) * D + h * DK;
@@ -637,9 +472,9 @@ __global__ void __launch_bounds__(NW * 32, 16 / NW) dec_src_attn_flash_kernel(co
   }
   cp_async_wait<0>();
   __syncthreads();
-  // ---- merge of the NW warps: red[warp][slot 16][66] = (O[64], m, l) in the ring
+  // ---- merge of the FLASH_NW warps: red[warp][slot 16][66] = (O[64], m, l) in the ring
   float* red = ring;
-  static_assert(S * STAGE_F >= NW * 16 * 66, "merge scratch must fit in the ring");
+  static_assert(S * STAGE_F >= FLASH_NW * 16 * 66, "merge scratch must fit in the ring");
   l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
   l0 += __shfl_xor_sync(0xffffffffu, l0, 2); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
 #pragma unroll
@@ -658,10 +493,10 @@ __global__ void __launch_bounds__(NW * 32, 16 / NW) dec_src_attn_flash_kernel(co
     const int w = i / DK, d = i % DK;
     float M = -INFINITY;
 #pragma unroll
-    for (int ww = 0; ww < NW; ++ww) M = fmaxf(M, red[((long long)ww * 16 + w) * 66 + 64]);
+    for (int ww = 0; ww < FLASH_NW; ++ww) M = fmaxf(M, red[((long long)ww * 16 + w) * 66 + 64]);
     float L = 0.f, a = 0.f;
 #pragma unroll
-    for (int ww = 0; ww < NW; ++ww) {
+    for (int ww = 0; ww < FLASH_NW; ++ww) {
       const float* r = red + ((long long)ww * 16 + w) * 66;
       const float e = expf(r[64] - M);      // a warp without frames: exp(-inf) = 0
       L = fmaf(r[65], e, L);
@@ -1198,7 +1033,7 @@ int espb_dec_self_attn_f32(const float* qkv, float* kc, float* vc, const int* an
   const size_t smem = (size_t)warps * sc_ld * sizeof(float);
   if (smem > 48 * 1024) { espb_set_error("dec_self_attn: prefix too long for the score buffer"); return ESPB_ERR_ARG; }
   const bool fast64 = (D / H == 64) && (D % 4 == 0) && (ctx_plane % 4 == 0) && ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(kc) |
-                       reinterpret_cast<uintptr_t>(vc) | reinterpret_cast<uintptr_t>(ctx)) & 15) == 0 && !getenv("ESPB_SELF_ATTN_GENERIC");
+                       reinterpret_cast<uintptr_t>(vc) | reinterpret_cast<uintptr_t>(ctx)) & 15) == 0;
   if (fast64)
     espb::launch_pdl(dec_self_attn64_kernel, dim3((n * H + warps - 1) / warps), dim3(warps * 32), smem, stream, qkv, kc, vc, anc, anc_ld, n, D, H, pos,
                      step_ptr, sc_ld, ctx, ctx_plane);
@@ -1217,63 +1052,26 @@ int espb_dec_src_attn_f32(const float* q, const float* kmem, const float* vmem, 
   while (lpr * 4 < dk) lpr <<= 1;
   for (int w0 = 0; w0 < W; w0 += 16) {   // the kernels keep <= 16 beam slots per block; wider beams stream K/V once per group of 16
     const int Wg = (W - w0 < 16) ? W - w0 : 16;
-    if (dk == 64 && !getenv("ESPNET_B200_SRC_ATTN_FFMA") && !getenv("ESPNET_B200_SRC_ATTN_TWOPASS")) {
-      // single-pass kernel: 3 stages of (K, V) tiles = 112 KB -> two blocks per SM, 128 KB of loads in flight per SM
-      using FlashFn = void (*)(const float*, const float*, const float*, int, const int*, int, int, int, float*, long long, int, int);
-      // NW = 4 (default): four 57 KB blocks per SM -- 528 resident on an H100's 132 SMs, so a 64-utterance x 8-head launch is one wave; NW = 8
-      // (ESPB_SRC_ATTN_NW=8, the first version): two 112 KB blocks per SM.  Same bytes in flight per SM.
-      static int nw = 0;
-      if (!nw) { const char* e = getenv("ESPB_SRC_ATTN_NW"); nw = (e && e[0] == '8') ? 8 : (e && e[0] == '4') ? 4 : ESPB_SRC_ATTN_NW_DEFAULT; }
-      const FlashFn fn = (nw == 4) ? dec_src_attn_flash_kernel<3, 4> : dec_src_attn_flash_kernel<3, 8>;
-      const size_t smem = (16 * 68 + 3 * 2 * 8 * nw * 68) * sizeof(float);
+    if (dk == 64) {
+      // single-pass kernel: 3 stages of (K, V) tiles; four blocks per SM -- 528 resident on an H100's 132 SMs, so a 64-utterance x 8-head
+      // launch is one wave
+      const size_t smem = (16 * 68 + 3 * 2 * 8 * FLASH_NW * 68) * sizeof(float);
       static bool attr = false;
       if (!attr) {
-        if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+        if (cudaFuncSetAttribute(dec_src_attn_flash_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
           espb_set_error("dec_src_attn: cannot raise dynamic shared memory"); return ESPB_ERR_CUDA;
         }
         attr = true;
       }
-      espb::launch_pdl(fn, dim3(U * H), dim3(nw * 32), smem, stream, q, kmem, vmem, Tmax, lens, Wg, D, H, ctx, ctx_plane, w0, W);
+      espb::launch_pdl(dec_src_attn_flash_kernel<3>, dim3(U * H), dim3(FLASH_NW * 32), smem, stream, q, kmem, vmem, Tmax, lens, Wg, D, H, ctx, ctx_plane,
+                       w0, W);
       ESPB_CHECK_LAUNCH();
       continue;
-    }
-    if (dk == 64 && !getenv("ESPNET_B200_SRC_ATTN_FFMA")) {   // two-pass variant (scores of the whole utterance in smem), kept for A/B
-      const size_t scs4 = ((size_t)Wg * Tmax + 3) & ~(size_t)3;
-      const size_t fixed = (16 * 68 + scs4) * sizeof(float), tile_b = 64 * 72 * sizeof(float);
-      // deepest ring that still lets two blocks share an SM (227 KB), else the deepest that fits one block
-      int S = 0;
-      for (int cand = 4; cand >= 2 && !S; --cand) if (fixed + cand * tile_b <= 113 * 1024) S = cand;
-      for (int cand = 4; cand >= 2 && !S; --cand) if (fixed + cand * tile_b <= 200 * 1024) S = cand;
-      if (S) {
-        using MmaFn = void (*)(const float*, const float*, const float*, int, const int*, int, int, int, float*, long long, int, int);
-        const MmaFn fn = (S == 4) ? dec_src_attn_mma_kernel<4> : (S == 3) ? dec_src_attn_mma_kernel<3> : dec_src_attn_mma_kernel<2>;
-        static bool attr[5] = {false, false, false, false, false};
-        if (!attr[S]) {
-          if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024)) != cudaSuccess) {
-            espb_set_error("dec_src_attn: cannot raise dynamic shared memory"); return ESPB_ERR_CUDA;
-          }
-          attr[S] = true;
-        }
-        espb::launch_pdl(fn, dim3(U * H), dim3(256), fixed + S * tile_b, stream, q, kmem, vmem, Tmax, lens, Wg, D, H, ctx, ctx_plane, w0, W);
-        ESPB_CHECK_LAUNCH();
-        continue;
-      }
     }
     const size_t red = (size_t)8 * Wg * dk, scs = ((size_t)Wg * Tmax + 3) & ~(size_t)3;
     const size_t smem = ((size_t)Wg * dk + (scs > red ? scs : red) + (size_t)128 * (dk + 4)) * sizeof(float);
     if (smem > 200 * 1024) { espb_set_error("dec_src_attn: beam*T too large for shared memory"); return ESPB_ERR_ARG; }
-    using KernelFn = void (*)(const float*, const float*, const float*, int, const int*, int, int, int, int, float*, long long, int, int);
-    KernelFn fn = dec_src_attn_kernel<4, 0, 0>;
-    if (dk == 64) {
-      switch (Wg) {
-        case 4: fn = dec_src_attn_kernel<4, 4, 64>; break;
-        case 5: fn = dec_src_attn_kernel<4, 5, 64>; break;
-        case 8: fn = dec_src_attn_kernel<4, 8, 64>; break;
-        case 10: fn = dec_src_attn_kernel<4, 10, 64>; break;
-        case 16: fn = dec_src_attn_kernel<4, 16, 64>; break;
-        default: break;
-      }
-    }
+    const auto fn = dec_src_attn_kernel<4>;
     if (smem > 48 * 1024) {
       if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024)) != cudaSuccess) {
         espb_set_error("dec_src_attn: cannot raise dynamic shared memory"); return ESPB_ERR_CUDA;

@@ -133,7 +133,7 @@ if which in ("ac", "all"):
                             sc=(T * Tp, H * T * Tp), b_off=D), alg)
 
 if which in ("logsoftmax", "all"):
-    # decode-step shape (640 hypotheses x V 5000) and the encoder-side CTC posteriors (64 x 937 frames); ESPB_LOGSOFTMAX_3PASS=1 = the first kernel
+    # decode-step shape (640 hypotheses x V 5000) and the encoder-side CTC posteriors (64 x 937 frames)
     for rows in (640, 64 * 937):
         x = torch.randn(rows, 5000, device=dev)
         timeit(f"log_softmax_rows {rows} x 5000", lambda: call("espb_log_softmax_rows_f32", ptr(x), rows, 5000, 5000), 2 * rows * 5000 * 4)

@@ -1,6 +1,6 @@
-"""The frontend kernels (csrc/frontend.cu) one by one through the C ABI: espb_stft_logmel_f32 (and the round-1 kernel behind ESPB_STFT_V1),
-espb_frontend_blocks, espb_utt_mvn_from_partial_f32, espb_utt_mvn_f32 and espb_global_mvn_f32.  The GPU tests carry pytest.mark.gpu one
-by one; the CPU tests of this file run anywhere.
+"""The frontend kernels (csrc/frontend.cu) one by one through the C ABI: espb_stft_logmel_f32, espb_frontend_blocks,
+espb_utt_mvn_from_partial_f32, espb_utt_mvn_f32 and espb_global_mvn_f32.  The GPU tests carry pytest.mark.gpu one by one; the CPU tests
+of this file run anywhere.
 
 Reference, per utterance, float64 numpy: reflect-pad the samples < len by 256 on both sides (torch.stft center=True), take frame t at
 t*hop, multiply by the float32 window the kernel receives (win_length taps zero-padded around the centre to 512, built by
@@ -11,7 +11,7 @@ elements past the outputs must stay NaN.
 Tolerance of the log-mel features, per element, u = 2^-24.
 * FFT.  The kernel packs the windowed frame into 256 complex points (one rounding per product x w), runs a 16 x 16 four-step FFT (two
   16-point DFTs of two radix-4 levels each with a twiddle multiplication between them, and the W256 twiddles between the DFTs) and the
-  real-FFT split (add, product with a float32 W512 twiddle, add); the round-1 kernel's four radix-4 Stockham stages have the same count.
+  real-FFT split (add, product with a float32 W512 twiddle, add).
   Each add level rounds once, each product with a float32 twiddle carries 2 roundings and the twiddle's own error: 23 roundings on any
   path.  Each level maps the vector by a matrix that is sqrt(r) times unitary, so a level's rounding errors reach X with an L2 norm of
   at most u sqrt(2 * 256) ||w x||_2 (complex components), and one element of X is bounded by the L2 norm of the error vector:
@@ -23,8 +23,8 @@ Tolerance of the log-mel features, per element, u = 2^-24.
   |exp(got) - max(M, 1e-10f)| <= dM + 3u |got| exp(got).  Where M + dM < 1e-10f the element must be ln(1e-10f) within 1 ulp (digital
   silence, filters with no non-zero bin).
 * partial[b][blk][m] is the sum of the kernel's own log-mel rows < Tf in frames [32 blk, 32 blk + 32): each half warp sums its 4 frames
-  (8 in the round-1 kernel) and the block adds at most 8 such sums, so it is within (32 + 8) u sum |x| of the float64 column sum; blocks
-  with no frame < Tf are exactly 0.
+  and the block adds at most 8 such sums, so it is within (32 + 8) u sum |x| of the float64 column sum; blocks with no frame < Tf are
+  exactly 0.
 * UtteranceMVN: the mean adds the nblk block sums in sequence and divides once, y = x - mean rounds once:
   tol = (40 + nblk + 2) u sum_t |x_t| / Tf + u |y|, against float64 mean subtraction of the kernel's own features.
 * GlobalMVN is compared bit for bit with the reference's float32 op order (oracle.frontend.global_mvn).
@@ -305,30 +305,6 @@ def test_stft_logmel_refusals(bad, match):
               _ptr(out), 32, _ptr(part))
     torch.cuda.synchronize()
     assert _all_nan_bits(out) and _all_nan_bits(part)
-
-
-@gpu
-@pytest.mark.parametrize("signal", [_noise, _tone, _silence], ids=lambda f: f.__name__[1:])
-@pytest.mark.parametrize("n_mels", [80, 96])
-def test_stft_v1_kernel(n_mels, signal, monkeypatch):
-    """ESPB_STFT_V1 (read on every call) selects the round-1 kernel at hop 128 and n_mels <= 96: same reference, poisoning and partials."""
-    monkeypatch.setenv("ESPB_STFT_V1", "1")
-    _case(128, SHORT[:2] + TF_EDGES[1:4] + [9001], signal=signal, seed=n_mels, n_mels=n_mels)
-
-
-@gpu
-@pytest.mark.parametrize("hop,n_mels", [(128, 97), (128, 128), (160, 80)])
-def test_stft_v1_variable_falls_back(hop, n_mels, monkeypatch):
-    """Where the round-1 kernel does not apply, ESPB_STFT_V1 changes nothing: the same bits as without it."""
-    fe, c = _tables("cuda", hop_length=hop, n_mels=n_mels)
-    rng = np.random.default_rng(hop + n_mels)
-    lens = [9001, 4097, 6400]
-    waves = [_noise(rng, n) for n in lens]
-    base = _stft(c, n_mels, hop, waves, lens, off=1)
-    monkeypatch.setenv("ESPB_STFT_V1", "1")
-    v1 = _stft(c, n_mels, hop, waves, lens, off=1)
-    for a, b in zip(base, v1):
-        assert np.array_equal(a.view(np.int32), b.view(np.int32))
 
 
 # ============================================================================================================== UtteranceMVN

@@ -20,9 +20,6 @@ Tolerances:
   m + log(sum) rounds once: tol = 4u (max|term| + |psi|) + 4u (n_seq + 8) + 1e-6.  part = psi - s_prev adds 2u (|psi| + |s_prev|).
 * log-softmax: the row's log-sum-exp is off by (V/256 + 16) 2u (256 threads, V/256 sequential adds each, tree reduction), the subtraction
   rounds once: tol = (V/256 + 16) 2u + 4u |out|.
-
-Not covered here: ESPB_SRC_ATTN_NW=8 and ESPB_LOGSOFTMAX_3PASS select A/B kernel variants once per process, so they cannot be switched per
-test; the three-pass log-softmax kernel itself runs for V > 8192.
 """
 import math
 
@@ -137,9 +134,9 @@ def _check_src(dk, H, W, lens, Tmax, seed):
         assert e < 2e-5, f"d_k {dk} W {W} utterance {u} (T {T}): max abs err {e:.3e}"
 
 
-def _src_lens_for(Wg, dk, ffma):
-    """The 2812-frame batch unless the FFMA kernel (the only path for d_k != 64, or forced) cannot hold its [W][Tmax] scores."""
-    if ffma and not _ffma_fits(Wg, dk, max(SRC_LENS) + 1):
+def _src_lens_for(Wg, dk):
+    """The 2812-frame batch unless the FFMA kernel (the path for d_k != 64) cannot hold its [W][Tmax] scores."""
+    if dk != 64 and not _ffma_fits(Wg, dk, max(SRC_LENS) + 1):
         return SRC_LENS_SHORT
     return SRC_LENS
 
@@ -149,32 +146,13 @@ def _src_lens_for(Wg, dk, ffma):
 def test_src_attn_default_path_vs_fp64(dk, H, W):
     """Default dispatch: the single-pass mma kernel at d_k = 64, the run-time FFMA kernel otherwise; slot groups of 16 with w0 > 0 and a
     partial last group for W > 16."""
-    lens = _src_lens_for(min(W, 16), dk, ffma=(dk != 64))
+    lens = _src_lens_for(min(W, 16), dk)
     _check_src(dk, H, W, lens, max(lens) + 1, seed=dk * 100 + W)
 
 
-# Wg = 16 slots: S = 4 while 16 Tmax <= 9408, S = 3 up to 14016, S = 2 up to 18624 (two blocks per SM); 1500 frames take the one-block S = 4.
-@pytest.mark.parametrize("W", [16, 20])
-@pytest.mark.parametrize("Tmax", [500, 800, 1100, 1500])
-def test_src_attn_twopass_vs_fp64(Tmax, W, monkeypatch):
-    monkeypatch.setenv("ESPNET_B200_SRC_ATTN_TWOPASS", "1")
-    lens = [1, 7, 63, 64, 65, Tmax - 1]
-    _check_src(64, 2, W, lens, Tmax, seed=Tmax + W)
-
-
-@pytest.mark.parametrize("W", [4, 5, 8, 10, 16, 7])
-def test_src_attn_ffma_forced_vs_fp64(W, monkeypatch):
-    """Compile-time W = 4, 5, 8, 10, 16 instances at d_k = 64, and the run-time-W kernel (W = 7)."""
-    monkeypatch.setenv("ESPNET_B200_SRC_ATTN_FFMA", "1")
-    lens = _src_lens_for(W, 64, ffma=True)
-    _check_src(64, 2, W, lens, max(lens) + 1, seed=700 + W)
-
-
-@pytest.mark.parametrize("dk,H,Tmax,force", [(32, 2, 3200, False), (48, 2, 2813, False), (128, 2, 2813, False), (64, 2, 2813, True)])
-def test_src_attn_refuses_beyond_shared_memory(dk, H, Tmax, force, monkeypatch):
+@pytest.mark.parametrize("dk,H,Tmax", [(32, 2, 3200), (48, 2, 2813), (128, 2, 2813)])
+def test_src_attn_refuses_beyond_shared_memory(dk, H, Tmax):
     """Past the FFMA kernel's shared-memory cap the launcher returns an error and launches nothing."""
-    if force:
-        monkeypatch.setenv("ESPNET_B200_SRC_ATTN_FFMA", "1")
     W = 16
     assert not _ffma_fits(W, dk, Tmax)
     lens = [Tmax] if Tmax == 3200 else [1, Tmax - 1]
@@ -212,17 +190,15 @@ def _ancestors(n, pos, rng, anc_ld, step_form):
     return anc
 
 
-SELF_KERNELS = [(64, 2, "fast"), (64, 2, "env"), (64, 2, "misaligned"), (16, 4, ""), (32, 3, ""), (48, 2, ""), (128, 2, "")]
+SELF_KERNELS = [(64, 2, "fast"), (64, 2, "misaligned"), (16, 4, ""), (32, 3, ""), (48, 2, ""), (128, 2, "")]
 
 
 @pytest.mark.parametrize("step_form", [False, True])
 @pytest.mark.parametrize("pos", [0, 1, 7, 8, 31, 32, 33, 64, 100])
 @pytest.mark.parametrize("dk,H,variant", SELF_KERNELS)
-def test_dec_self_attn_vs_fp64(dk, H, variant, pos, step_form, monkeypatch):
-    """The d_k = 64 kernel, the generic kernel (d_k 16 / 32 / 48 / 128, and d_k = 64 forced through ESPB_SELF_ATTN_GENERIC or a ctx
-    pointer off 16-byte alignment) over a cache gathered through a random ancestor table; the position as a value or value + *step_ptr."""
-    if variant == "env":
-        monkeypatch.setenv("ESPB_SELF_ATTN_GENERIC", "1")
+def test_dec_self_attn_vs_fp64(dk, H, variant, pos, step_form):
+    """The d_k = 64 kernel, the generic kernel (d_k 16 / 32 / 48 / 128, and d_k = 64 with a ctx pointer off 16-byte alignment) over a cache
+    gathered through a random ancestor table; the position as a value or value + *step_ptr."""
     rng = np.random.default_rng(1000 * dk + 10 * pos + step_form)
     n, D = 6, H * dk
     max_pos = pos + 3 if step_form else pos
