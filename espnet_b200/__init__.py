@@ -18,7 +18,7 @@ from .errors import TooShortUttError  # noqa: F401
 from .frontend import DefaultFrontend, GlobalMVN, LogMel, UtteranceMVN  # noqa: F401
 from .rnn_decoder import RNNDecoder  # noqa: F401
 from .rnn_encoder import RNNEncoder, VGGRNNEncoder  # noqa: F401
-from .lm import SequentialRNNLM, TransformerLM, build_lm_from_file  # noqa: F401
+from .lm import ESPnetLanguageModel, SequentialRNNLM, TransformerLM, build_espnet_lm_from_file, build_lm_from_file  # noqa: F401
 from .search import BatchBeamSearch, Hypothesis  # noqa: F401
 from .search_online import BatchBeamSearchOnline, LengthBonus  # noqa: F401
 from .asr_inference_streaming import Speech2TextStreaming  # noqa: F401

@@ -44,6 +44,7 @@ struct AttnParams {
   float* out; long long out_plane, ldo;          // split context [rows][H*DK]
   int B, H, T, nqb;                              // nqb = ceil(T / 128)
   float scale;                                   // 1 / sqrt(d_k)
+  const int* tok;                                // causal attention: token ids [B][T]; key j is valid iff tok[b][j] != 0
 };
 
 // bd values of one row for the keys key0 + 8j + 0/1, j < 8 (key0 even; row = the row's bd pointer shifted by T-1-i): pairs as one 8-byte
@@ -67,7 +68,10 @@ __device__ __forceinline__ void load_bd_row(const float* row, int key0, int len,
   }
 }
 
-template <bool RELPOS>
+// CAUSAL (TransformerLM._target_mask, transformer_lm.py:57-60): query i attends the keys j <= i (and j < len) whose token id is not 0.  A
+// CTA loads only the key tiles up to its last query row; warpgroup 0 skips the MMAs of the tile wholly above its 64 rows.  A row without a
+// valid key gets a zero output, as the reference's masked_fill(mask, 0.0) after the softmax gives.
+template <bool RELPOS, bool CAUSAL>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 flash_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                   AttnParams p) {
@@ -85,7 +89,7 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
   const int qb = item % p.nqb, h = (item / p.nqb) % p.H, b = item / (p.nqb * p.H);
   const int len = min(p.lens[b], p.T);
   const int I0 = qb * QB;                      // first query row of the CTA
-  const int nkt = (len + KB - 1) / KB;
+  const int nkt = ((CAUSAL ? min(len, I0 + QB) : len) + KB - 1) / KB;
 
   if (I0 >= len || nkt == 0) {
     // every query row of this block is padding (t >= len): defined (zero) output, no tensor work
@@ -170,6 +174,15 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
     const int st = t % KV_STAGES;
     const uint32_t ph = (uint32_t)((t / KV_STAGES) & 1);
     const int J0 = t * KB;
+    if (CAUSAL && J0 > I0 + g * 64 + 63) {
+      // every key of the tile lies above this warpgroup's diagonal: release the stages once they are full (the producer refilled them only
+      // after the other warpgroup released the tile before), no MMA
+      mbar_wait_spin(k_full + 8 * st, ph);
+      if ((threadIdx.x & 127) == 0) mbar_arrive_local(k_empty + 8 * st);
+      mbar_wait_spin(v_full + 8 * st, ph);
+      if ((threadIdx.x & 127) == 0) mbar_arrive_local(v_empty + 8 * st);
+      continue;
+    }
     if (RELPOS) {
       load_bd_row(bd_a, J0 + 2 * tq, len, bdv_a);
       load_bd_row(bd_b, J0 + 2 * tq, len, bdv_b);
@@ -204,6 +217,11 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
         const int key = J0 + 8 * j + 2 * tq + e;
         const bool ok = key < len;
         float va = s[4 * j + e], vb = s[4 * j + 2 + e];
+        if (CAUSAL) {
+          const bool kv = ok && __ldg(p.tok + (long long)b * p.T + key) != 0;
+          va = kv && key <= ra ? va : -INFINITY;
+          vb = kv && key <= rb ? vb : -INFINITY;
+        }
         if (RELPOS) {
           if (ok && bd_a) va += e ? bdv_a[j].y : bdv_a[j].x;
           if (ok && bd_b) vb += e ? bdv_b[j].y : bdv_b[j].x;
@@ -217,14 +235,17 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
     mt_a = fmaxf(mt_a, __shfl_xor_sync(0xffffffffu, mt_a, 1)); mt_a = fmaxf(mt_a, __shfl_xor_sync(0xffffffffu, mt_a, 2));
     mt_b = fmaxf(mt_b, __shfl_xor_sync(0xffffffffu, mt_b, 1)); mt_b = fmaxf(mt_b, __shfl_xor_sync(0xffffffffu, mt_b, 2));
     const float mn_a = fmaxf(m_a, mt_a * scale), mn_b = fmaxf(m_b, mt_b * scale);   // scale > 0: max commutes with the scaling
-    const float al_a = __expf(m_a - mn_a), al_b = __expf(m_b - mn_b);              // first tile: exp(-inf) = 0
+    // the max the exponentials subtract: with no valid key so far (causal rows whose keys are all masked) 0 instead of -inf, so that
+    // exp(-inf - max) is 0 and not NaN
+    const float mu_a = CAUSAL && mn_a == -INFINITY ? 0.f : mn_a, mu_b = CAUSAL && mn_b == -INFINITY ? 0.f : mn_b;
+    const float al_a = __expf(m_a - mu_a), al_b = __expf(m_b - mu_b);              // first tile: exp(-inf) = 0
     float ls_a = 0.f, ls_b = 0.f;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
-        s[4 * j + e] = __expf(fmaf(s[4 * j + e], scale, -mn_a));           // masked: exp(-inf) = 0
-        s[4 * j + 2 + e] = __expf(fmaf(s[4 * j + 2 + e], scale, -mn_b));
+        s[4 * j + e] = __expf(fmaf(s[4 * j + e], scale, -mu_a));           // masked: exp(-inf) = 0
+        s[4 * j + 2 + e] = __expf(fmaf(s[4 * j + 2 + e], scale, -mu_b));
         ls_a += s[4 * j + e]; ls_b += s[4 * j + 2 + e];
       }
     }
@@ -273,7 +294,7 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
   // ---- total row sums over the quad, normalise, store hi / lo
   l_a += __shfl_xor_sync(0xffffffffu, l_a, 1); l_a += __shfl_xor_sync(0xffffffffu, l_a, 2);
   l_b += __shfl_xor_sync(0xffffffffu, l_b, 1); l_b += __shfl_xor_sync(0xffffffffu, l_b, 2);
-  const float inv_a = 1.f / l_a, inv_b = 1.f / l_b;
+  const float inv_a = CAUSAL && l_a == 0.f ? 0.f : 1.f / l_a, inv_b = CAUSAL && l_b == 0.f ? 0.f : 1.f / l_b;
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const int row = r ? rb : ra;
@@ -290,38 +311,28 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
   }
 }
 
-template <bool RELPOS>
+template <bool RELPOS, bool CAUSAL>
 int launch_flash(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const AttnParams& p, cudaStream_t stream) {
   constexpr int smem = Q_BYTES + 2 * KV_STAGES * KV_STAGE_BYTES + 1024 + 256;
   static_assert(smem <= 232448, "dynamic shared memory budget exceeded");
   static bool attr_set = false;
   if (!attr_set) {
-    if (cudaFuncSetAttribute(flash_attn_kernel<RELPOS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
+    if (cudaFuncSetAttribute(flash_attn_kernel<RELPOS, CAUSAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
       espb_set_error("cudaFuncSetAttribute(max dynamic smem) failed (flash attention)");
       return ESPB_ERR_CUDA;
     }
     attr_set = true;
   }
   const long long items = (long long)p.B * p.H * p.nqb;
-  flash_attn_kernel<RELPOS><<<dim3((unsigned)items), ATT_THREADS, smem, stream>>>(tmQ, tmK, tmV, p);
+  flash_attn_kernel<RELPOS, CAUSAL><<<dim3((unsigned)items), ATT_THREADS, smem, stream>>>(tmQ, tmK, tmV, p);
   ESPB_CHECK_LAUNCH();
   return ESPB_OK;
 }
 
-}  // namespace
-
-extern "C" {
-
-// Fused (rel-pos) self-attention for d_k = 64.  All tensors are device fp32.
-//   q       split [2][B*T][ldq] (planes q_plane apart; first element at q + q_off): query rows (q + pos_bias_u for rel-pos attention);
-//           head h at columns h*64..
-//   k       split, same layout convention (k_off, k_plane, ldk): key rows;  vt split [2][B][H][64][Tp]: V transposed, keys >= len zero
-//   bd      [B][H][T][Rp] unshifted (q + pos_bias_v) p^T (columns 0..2T-2), or NULL for plain attention
-//   out     split [2][B*T][ldo]: context, head h at columns h*64..
-int espb_flash_attn_f32(const float* q, long long q_off, long long q_plane, long long ldq, const float* k, long long k_off, long long k_plane,
-                        long long ldk, const float* vt, long long vt_plane, int Tp, const float* bd, int Rp, const int* lens, int B, int H, int T,
-                        int dk, float* out, long long out_plane, long long ldo, cudaStream_t stream) {
-  q += q_off; k += k_off;
+// Tensor maps and parameters shared by the two entry points; tok != nullptr selects the causal kernel (bd is then null).
+int flash_entry(const float* q, long long q_plane, long long ldq, const float* k, long long k_plane, long long ldk, const float* vt,
+                long long vt_plane, int Tp, const float* bd, int Rp, const int* tok, const int* lens, int B, int H, int T, int dk, float* out,
+                long long out_plane, long long ldo, cudaStream_t stream) {
   if (dk != DK) { espb_set_error("flash_attn: d_k must be 64"); return ESPB_ERR_ARG; }
   if (B <= 0 || H <= 0 || T <= 0) { espb_set_error("flash_attn: bad shape"); return ESPB_ERR_ARG; }
   if ((ldq & 3) || (q_plane & 3) || (ldo & 3) || (out_plane & 3) || (reinterpret_cast<uintptr_t>(q) & 15) || (reinterpret_cast<uintptr_t>(out) & 15)) {
@@ -347,9 +358,36 @@ int espb_flash_attn_f32(const float* q, long long q_off, long long q_plane, long
   }
   AttnParams p;
   p.q = q; p.q_plane = q_plane; p.ldq = ldq; p.lens = lens; p.bd = bd; p.Rp = Rp; p.out = out; p.out_plane = out_plane; p.ldo = ldo;
-  p.B = B; p.H = H; p.T = T; p.nqb = (T + QB - 1) / QB; p.scale = 1.0f / sqrtf((float)dk);
-  if (bd) return launch_flash<true>(tmQ, tmK, tmV, p, stream);
-  return launch_flash<false>(tmQ, tmK, tmV, p, stream);
+  p.B = B; p.H = H; p.T = T; p.nqb = (T + QB - 1) / QB; p.scale = 1.0f / sqrtf((float)dk); p.tok = tok;
+  if (tok) return launch_flash<false, true>(tmQ, tmK, tmV, p, stream);
+  if (bd) return launch_flash<true, false>(tmQ, tmK, tmV, p, stream);
+  return launch_flash<false, false>(tmQ, tmK, tmV, p, stream);
+}
+
+}  // namespace
+
+extern "C" {
+
+// Fused (rel-pos) self-attention for d_k = 64.  All tensors are device fp32.
+//   q       split [2][B*T][ldq] (planes q_plane apart; first element at q + q_off): query rows (q + pos_bias_u for rel-pos attention);
+//           head h at columns h*64..
+//   k       split, same layout convention (k_off, k_plane, ldk): key rows;  vt split [2][B][H][64][Tp]: V transposed, keys >= len zero
+//   bd      [B][H][T][Rp] unshifted (q + pos_bias_v) p^T (columns 0..2T-2), or NULL for plain attention
+//   out     split [2][B*T][ldo]: context, head h at columns h*64..
+int espb_flash_attn_f32(const float* q, long long q_off, long long q_plane, long long ldq, const float* k, long long k_off, long long k_plane,
+                        long long ldk, const float* vt, long long vt_plane, int Tp, const float* bd, int Rp, const int* lens, int B, int H, int T,
+                        int dk, float* out, long long out_plane, long long ldo, cudaStream_t stream) {
+  return flash_entry(q + q_off, q_plane, ldq, k + k_off, k_plane, ldk, vt, vt_plane, Tp, bd, Rp, nullptr, lens, B, H, T, dk, out, out_plane, ldo,
+                     stream);
+}
+
+// Causal self-attention of the Transformer LM, same layouts as espb_flash_attn_f32 without bd; tok [B][T] int32 token ids.
+int espb_causal_flash_attn_f32(const float* q, long long q_off, long long q_plane, long long ldq, const float* k, long long k_off,
+                               long long k_plane, long long ldk, const float* vt, long long vt_plane, int Tp, const int* tok, const int* lens, int B,
+                               int H, int T, int dk, float* out, long long out_plane, long long ldo, cudaStream_t stream) {
+  if (!tok) { espb_set_error("causal_flash_attn: tok must not be NULL"); return ESPB_ERR_ARG; }
+  return flash_entry(q + q_off, q_plane, ldq, k + k_off, k_plane, ldk, vt, vt_plane, Tp, nullptr, 0, tok, lens, B, H, T, dk, out, out_plane, ldo,
+                     stream);
 }
 
 }  // extern "C"

@@ -90,6 +90,9 @@ _SIGS = {
     "espb_rnn_proj_post_f32": [P, I, I, I, P, I, I, P, L, I, P],
     "espb_drop_cand_i32": [P, I, I, I, P],
     "espb_att_loc_step_f32": [P, P, L, P, I, I, I, I, P, P, I, I, P, P, P, P, I, I, P, P, I, P, L, I, P, L, I, P],
+    "espb_causal_flash_attn_f32": [P, L, L, L, P, L, L, L, P, L, I, P, P, I, I, I, I, P, L, L, P],
+    "espb_causal_softmax_f32": [P, I, I, I, I, P, P, F, P, L, P],
+    "espb_nll_rows_f32": [P, L, L, I, P, P, P],
 }
 
 ABI_VERSION = 7   # espb_abi_version() of the library this binding matches (include/espnet_b200.h)

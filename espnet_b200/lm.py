@@ -8,6 +8,9 @@ names, so a reference LM checkpoint (``ESPnetLanguageModel`` state_dict, keys ``
 Like the decoder (decoder.py) the new token of every hypothesis is scored against a position-major K / V cache addressed through the search's
 ancestor table, instead of re-running the prefix: the decode-step kernels without the cross-attention.
 
+Each LM also runs whole sentences (``forward`` / ``_logits``: the reference's forward, with the causal token-masked attention of
+transformer_lm.py:57-72 for the TransformerLM), and ``ESPnetLanguageModel`` computes their negative log-likelihood for perplexity.
+
 Limit: the reference masks prefix positions that hold token id 0 (``_target_mask``, transformer_lm.py:59-62: id 0 is the padding / blank id);
 beam hypotheses never contain it in joint or CTC decoding (the CTC prefix score of blank is log-zero) -- a hypothesis with an explicit token 0
 in attention-only decoding would be scored without that mask here.
@@ -19,7 +22,7 @@ import torch
 
 from . import ops
 from .decoder import KVCacheScorer, ScorerProtocol
-from .layers import LN_EPS, _FFN, _MHA, PackedModule
+from .layers import LN_EPS, _FFN, _MHA, PackedModule, _pitch
 from .lib import call, ptr
 from .ops import ACT_RELU, _count, layernorm, linear, split_from
 
@@ -105,6 +108,99 @@ class TransformerLM(KVCacheScorer):
             self._self_attn(x, xn, ctx, w, li, st, pos, anc, step_ptr)
             self._ffn(x, xn, w["n2"], w["ffn"], ACT_RELU)
         return self._head(x, xn, n)
+
+    # ---------------------------------------------------------------- full-sequence forward (perplexity)
+    def forward(self, input: torch.Tensor, hidden: None) -> Tuple[torch.Tensor, None]:
+        """transformer_lm.py:62-72: logits (B, L, V) of every position of input (B, L), keys masked by _target_mask (token id 0 and the
+        future)."""
+        return _forward_logits(self, input), None
+
+    @torch.no_grad()
+    def _logits(self, tok, lens32, B, T):
+        """Logits [B*T][V] (workspace) of token ids tok (B, T) int32 on the device: embedding, embed Linear + LayerNorm + ReLU (+ sinusoidal
+        positions), the layers with causal attention, after_norm, output projection.  Rows t >= lens32[b] are not defined."""
+        pk = self._packed or self._pack()
+        D, E, M = self.d, self.embed_unit, B * T
+        es = self._buf("es", (2, M, E))
+        x = self._buf("x", (M, D))
+        xn = self._buf("xn", (2, M, D))
+        ctx = self._buf("ctx", (2, M, D))
+        qkv = self._buf("qkv", (2, M, 3 * D))
+        ops.call("espb_gather_rows_split_f32", ops.ptr(tok), ops.ptr(pk["emb"]), M, E, ops.ptr(es), M * E)
+        _count()
+        linear(es, pk["in_w"], x, bias=pk["in_b"])
+        layernorm(x, pk["in_ln"][0], pk["in_ln"][1], pk["in_ln"][2], out_plain=x)
+        ops.call("espb_relu_posenc_f32", ops.ptr(x), M, D, None, 0, None, 1.0)   # ReLU
+        _count()
+        if self.pos_enc == "sinusoidal":   # PositionalEncoding: x * sqrt(D) + pe[t], each product rounded like the reference's
+            pe = self._pe(max(32, 1 << (T - 1).bit_length()))   # rows 0..T-1 of a power-of-two table: one table serves many lengths
+            for b in range(B):
+                xb = x[b * T:(b + 1) * T]
+                ops.call("espb_axpby_f32", ops.ptr(xb), math.sqrt(D), ops.ptr(pe), 1.0, ops.ptr(xb), T * D)
+            _count(B)
+        for w in pk["layers"]:
+            layernorm(x, *w["n1"], LN_EPS, out_split=xn)
+            linear(xn, w["qkv_w"], qkv, bias=w["qkv_b"], split_out=True)
+            self._causal_attn(qkv, ctx, tok, lens32, B, T)
+            linear(ctx, w["out_w"], x, bias=w["out_b"], residual=x)
+            self._ffn(x, xn, w["n2"], w["ffn"], ACT_RELU)
+        layernorm(x, *pk["an"], LN_EPS, out_split=xn)
+        logits = self._buf("logits", (M, self.vocab_size))
+        linear(xn, pk["out_w"], logits, bias=pk["out_b"])
+        return logits
+
+    def _causal_attn(self, qkv, ctx, tok, lens32, B, T):
+        """Causal self-attention with the token-0 key mask, from the fused q|k|v projection qkv (split [2][B*T][3D]) to ctx (split
+        [2][B*T][D]): the fused wgmma kernel for d_k = 64, else q k^T GEMM, masked softmax, p v GEMM."""
+        D, H = self.d, self.heads
+        dk, M, Tp = D // H, B * T, _pitch(T)
+        vt = self._buf("vt", (2, B, H, dk, Tp))
+        ops.call("espb_v_transpose_f32", ops.ptr(qkv), M * 3 * D, B, T, D, H, ops.ptr(lens32), ops.ptr(vt), B * H * dk * Tp, Tp)
+        _count()
+        if ops.use_flash_attn(dk):
+            ops.call("espb_causal_flash_attn_f32", ops.ptr(qkv), 0, M * 3 * D, 3 * D, ops.ptr(qkv), D, M * 3 * D, 3 * D, ops.ptr(vt),
+                     B * H * dk * Tp, Tp, ops.ptr(tok), ops.ptr(lens32), B, H, T, dk, ops.ptr(ctx), M * D, D)
+            _count()
+            return
+        sc, probs = self._buf("sc", (B, H, T, Tp)), self._buf("probs", (2, B, H, T, Tp))
+        ops.gemm(T, T, dk, qkv, M * 3 * D, 3 * D, qkv, M * 3 * D, 3 * D, sc, Tp, nbx=H, nby=B, sa=(dk, T * 3 * D), sb=(dk, T * 3 * D),
+                 sc=(T * Tp, H * T * Tp), b_off=D)
+        ops.call("espb_causal_softmax_f32", ops.ptr(sc), B, H, T, Tp, ops.ptr(lens32), ops.ptr(tok), math.sqrt(dk), ops.ptr(probs),
+                 B * H * T * Tp)
+        _count()
+        ops.gemm(T, dk, T, probs, B * H * T * Tp, Tp, vt, B * H * dk * Tp, Tp, ctx, D, c_plane=M * D, split_out=True, nbx=H, nby=B,
+                 sa=(T * Tp, H * T * Tp), sb=(dk * Tp, H * dk * Tp), sc=(dk, T * D))
+
+
+def _forward_logits(lm, input):
+    """forward(input, None) of either LM: every position of every row of input (B, L) is valid; a fresh (B, L, V) tensor."""
+    input = torch.as_tensor(input)
+    B, T = input.shape
+    if B == 0 or T == 0:
+        return torch.zeros(B, T, lm.vocab_size, dtype=torch.float32, device=lm._device)
+    tok = _check_ids(input, lm.vocab_size).to(device=lm._device, dtype=torch.int32).contiguous()
+    lens32 = torch.full((B,), T, dtype=torch.int32, device=tok.device)
+    with _ws_tag(lm, "seq"):
+        return lm._logits(tok, lens32, B, T).view(B, T, -1).clone()
+
+
+def _check_ids(ids, V):
+    if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= V):
+        raise IndexError(f"token ids must lie in [0, {V}) (got {int(ids.min())} .. {int(ids.max())})")
+    return ids
+
+
+class _ws_tag:
+    """Runs the full-sequence forward in a workspace set of its own, so that it neither reallocates nor overwrites the step scorer's."""
+
+    def __init__(self, m, tag):
+        self.m, self.tag = m, tag
+
+    def __enter__(self):
+        self.prev, self.m.ws_tag = self.m.ws_tag, self.tag
+
+    def __exit__(self, *exc):
+        self.m.ws_tag = self.prev
 
 
 def _pad4(k):
@@ -210,6 +306,47 @@ class SequentialRNNLM(ScorerProtocol, PackedModule):
         ops.log_softmax_rows_(logp)
         return logp
 
+    # ---------------------------------------------------------------- full-sequence forward (perplexity)
+    def forward(self, input: torch.Tensor, hidden: None) -> Tuple[torch.Tensor, None]:
+        """seq_rnn_lm.py:84-96 from the zero state: logits (B, L, V) of every position of input (B, L).  The final (h, c) is not returned
+        (None), and a given hidden state is refused."""
+        if hidden is not None:
+            raise NotImplementedError("espnet_b200 SequentialRNNLM.forward starts from the zero state (hidden=None)")
+        return _forward_logits(self, input), None
+
+    @torch.no_grad()
+    def _logits(self, tok, lens32, B, T):
+        """Logits [B*T][V] (workspace) of token ids tok (B, T) int32 on the device.  Per layer one GEMM of the inputs of all positions with
+        W_ih (+ both biases), then per step h W_hh^T and the cell (espb_lstm_rec_step_f32); utterance b stops at lens32[b] (its rows past
+        it are 0, as the padded steps of a unidirectional LSTM never reach the valid ones)."""
+        pk = self._packed or self._pack()
+        E, H, L, M = self.unit, self.nhid, self.nlayers, B * T
+        Ep, Hp = _pad4(E), _pad4(H)
+        kp0 = Ep + Hp
+        # layer 0's operand in the step layout [embedding | zero h] (pitch Ep + Hp, 16-byte rows for TMA); the K = Ep GEMM reads the
+        # embedding half.  The layer outputs alternate between two buffers; y[0] stands in for the h ring the gather does not read at pos 0.
+        xs = self._buf("seq_x0", (2, M, kp0), zero=True)
+        ys = [self._buf(f"seq_y{i}", (2, M, Hp), zero=True) for i in range(min(L, 2))]
+        ops.call("espb_rnnlm_gather_f32", ops.ptr(tok), ops.ptr(pk["emb"]), E, Ep, None, 0, 0, None, ops.ptr(ys[0]), 1, M, H, Hp, ops.ptr(xs))
+        _count()
+        xg, hg = self._buf("seq_xg", (M, 4 * H)), self._buf("seq_hg", (B, 4 * H))
+        h, c = self._buf("seq_h", (2, B, Hp), zero=True), self._buf("seq_c", (B, H))
+        for li, (w, bias) in enumerate(pk["layers"]):
+            ip = Ep if li == 0 else Hp
+            kp = ip + Hp
+            x, lda = (xs, kp0) if li == 0 else (ys[(li - 1) % 2], Hp)
+            y = ys[li % 2]
+            ops.gemm(M, 4 * H, ip, x, M * lda, lda, w, 4 * H * kp, kp, xg, 4 * H, bias=bias)
+            for s in range(T):
+                if s > 0:   # h_{s-1} W_hh^T: the recurrent half of the packed [W_ih | W_hh]
+                    ops.gemm(B, 4 * H, Hp, h, B * Hp, Hp, w, 4 * H * kp, kp, hg, 4 * H, b_off=ip)
+                ops.call("espb_lstm_rec_step_f32", ops.ptr(xg), ops.ptr(hg), ops.ptr(lens32), s, B, T, H, Hp, 1, ops.ptr(h), B * Hp, ops.ptr(c),
+                         ops.ptr(y), M * Hp, Hp)
+                _count()
+        logits = self._buf("logits", (M, self.vocab_size))
+        linear(ys[(L - 1) % 2], pk["out_w"], logits, bias=pk["out_b"])
+        return logits
+
     # ---------------------------------------------------------------- BatchScorerInterface (scorer_interface.py:85-188): per hypothesis (h, c)
     @torch.no_grad()
     def batch_score(self, ys: torch.Tensor, states: List[Any], xs: torch.Tensor) -> Tuple[torch.Tensor, List[Any]]:
@@ -250,3 +387,71 @@ def build_lm_from_file(config_file, model_file=None, device="cuda"):
         sd = torch.load(model_file, map_location="cpu")
         lm.load_state_dict({k[3:]: v for k, v in sd.items() if k.startswith("lm.")}, strict=True)
     return lm.to(device).eval(), args
+
+
+class ESPnetLanguageModel(torch.nn.Module):
+    """Drop-in container for espnet2.lm.espnet_model.ESPnetLanguageModel (inference): ``lm`` (so the checkpoint keys are ``lm.*``), sos = eos =
+    vocab_size - 1, ``nll`` and ``batchify_nll``.  The negative log-likelihood runs on the device: the LM's full-sequence logits, then one
+    kernel that reads each logit row once (espb_nll_rows_f32)."""
+
+    def __init__(self, lm: torch.nn.Module, vocab_size: int, ignore_id: int = 0):
+        super().__init__()
+        if not isinstance(lm, (TransformerLM, SequentialRNNLM)):
+            raise NotImplementedError(f"espnet_b200 ESPnetLanguageModel wraps TransformerLM and SequentialRNNLM (got {type(lm).__name__})")
+        self.lm = lm
+        self.sos = self.eos = vocab_size - 1
+        self.ignore_id = ignore_id
+
+    @torch.no_grad()
+    def nll(self, text: torch.Tensor, text_lengths: torch.Tensor, max_length: int = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """espnet_model.py:24-70: x = <eos> text, t = text <sos>; nll (B, L + 1) with 0 at positions >= text_lengths + 1, and text_lengths + 1."""
+        B = text.shape[0]
+        lens = torch.as_tensor(text_lengths).cpu().long()
+        text = text[:, : int(lens.max())] if max_length is None else text[:, : int(max_length)]
+        T = text.shape[1] + 1
+        x_lengths = torch.as_tensor(text_lengths) + 1
+        dev = self.lm._device
+        pos = torch.arange(T).view(1, T)
+        valid = pos < (lens + 1).view(B, 1)                     # positions whose nll the reference keeps
+        x = torch.zeros(B, T, dtype=torch.long)                 # positions past a sentence hold 0: they never reach a valid one
+        x[:, 0] = self.eos
+        x[:, 1:] = text.cpu()
+        x = torch.where(valid, x, torch.zeros_like(x))
+        tgt = torch.full((B, T), -1, dtype=torch.long)          # -1: written as 0 by the kernel
+        tgt[:, :-1] = text.cpu()
+        tgt[torch.arange(B), lens.clamp(max=T - 1)] = self.sos  # t[i, l] = sos
+        tgt = torch.where(valid, tgt, torch.full_like(tgt, -1))
+        if B == 0:
+            return torch.zeros(0, T, device=dev), x_lengths
+        _check_ids(x, self.lm.vocab_size)
+        _check_ids(tgt[valid], self.lm.vocab_size)
+        x32 = x.to(device=dev, dtype=torch.int32)
+        t32 = tgt.to(device=dev, dtype=torch.int32)
+        lens32 = (lens + 1).clamp(max=T).to(device=dev, dtype=torch.int32)
+        out = torch.empty(B, T, dtype=torch.float32, device=dev)
+        with _ws_tag(self.lm, "seq"):
+            logits = self.lm._logits(x32, lens32, B, T)
+            ops.call("espb_nll_rows_f32", ops.ptr(logits), B * T, logits.stride(0), self.lm.vocab_size, ops.ptr(t32), ops.ptr(out))
+            _count()
+        return out, x_lengths
+
+    def batchify_nll(self, text: torch.Tensor, text_lengths: torch.Tensor, batch_size: int = 100) -> Tuple[torch.Tensor, torch.Tensor]:
+        """espnet_model.py:72-114: nll in chunks of batch_size sentences, all padded to the longest."""
+        total = text.size(0)
+        if total <= batch_size:
+            return self.nll(text, text_lengths)
+        max_length = int(torch.as_tensor(text_lengths).max())
+        nlls, x_lengths = [], []
+        for start in range(0, total, batch_size):
+            n, xl = self.nll(text[start:start + batch_size], text_lengths[start:start + batch_size], max_length=max_length)
+            nlls.append(n)
+            x_lengths.append(xl)
+        return torch.cat(nlls), torch.cat(x_lengths)
+
+
+def build_espnet_lm_from_file(config_file, model_file=None, device="cuda"):
+    """LMTask.build_model_from_file returning the whole ESPnetLanguageModel (tasks/lm.py:173-210): build_lm_from_file's LM wrapped with the
+    config's model_conf."""
+    lm, args = build_lm_from_file(config_file, model_file, device)
+    model = ESPnetLanguageModel(lm, vocab_size=len(args.token_list), **(getattr(args, "model_conf", None) or {}))
+    return model.eval(), args

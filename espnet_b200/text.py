@@ -52,6 +52,10 @@ class CharTokenizer:
     def __repr__(self):
         return f'{self.__class__.__name__}(space_symbol="{self.space_symbol}")'
 
+    def text2tokens(self, line: str) -> List[str]:
+        """char_tokenizer.py:48-66 without non-linguistic symbols: one token per character, " " -> space_symbol."""
+        return [c if c != " " else self.space_symbol for c in line]
+
     def tokens2text(self, tokens: Iterable[str]) -> str:
         return "".join(t if t != self.space_symbol else " " for t in tokens)
 
@@ -62,6 +66,9 @@ class WordTokenizer:
 
     def __repr__(self):
         return f'{self.__class__.__name__}(delimiter="{self.delimiter}")'
+
+    def text2tokens(self, line: str) -> List[str]:
+        return line.split(self.delimiter)
 
     def tokens2text(self, tokens: Iterable[str]) -> str:
         return (" " if self.delimiter is None else self.delimiter).join(tokens)
@@ -83,6 +90,10 @@ class SentencepiecesTokenizer:
 
             self.sp = spm.SentencePieceProcessor()
             self.sp.load(self.model)
+
+    def text2tokens(self, line: str) -> List[str]:
+        self._build()
+        return self.sp.EncodeAsPieces(line)
 
     def tokens2text(self, tokens: Iterable[str]) -> str:
         self._build()

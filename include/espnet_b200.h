@@ -282,6 +282,23 @@ int espb_drop_cand_i32(int* valid, int n, int PC, int j, cudaStream_t stream);
 int espb_step_inc_i32(int* step, cudaStream_t stream);
 int espb_count_active_i32(const int* active, int n, int* out, cudaStream_t stream);
 
+/* ---- LM perplexity: full-sequence TransformerLM / SequentialRNNLM forward and ESPnetLanguageModel.nll (espnet2/lm/espnet_model.py:24-70,
+   espnet2/bin/lm_calc_perplexity.py) ---- */
+/* Causal self-attention of TransformerLM.forward for d_k = 64 (transformer_lm.py:57-72: _target_mask = (ys != 0) & subsequent_mask, through
+ * attention.py:153-265): out[b,i,h,:] = softmax_{j <= i, j < len_b, tok[b][j] != 0}( q[b,i,h,:] . k[b,j,h,:] / sqrt(d_k) ) . v[b,j,h,:], a row
+ * without a valid key 0.  Layouts and alignment as espb_flash_attn_f32 (no bd); tok [B][T] int32.  Each 128-query block reads only the
+ * key tiles up to its last row. */
+int espb_causal_flash_attn_f32(const float* q, long long q_off, long long q_plane, long long ldq, const float* k, long long k_off,
+                               long long k_plane, long long ldk, const float* vt, long long vt_plane, int Tp, const int* tok, const int* lens, int B,
+                               int H, int T, int dk, float* out, long long out_plane, long long ldo, cudaStream_t stream);
+/* The same mask for the materialised path (d_k != 64): probs = softmax(scores / sqrt_dk) over the keys j <= i, j < lens[b], tok[b][j] != 0,
+ * 0 elsewhere and on rows without a valid key; scores [B][H][T][Tp] -> probs hi/lo planes [B][H][T][Tp]. */
+int espb_causal_softmax_f32(const float* scores, int B, int H, int T, int Tp, const int* lens, const int* tok, float sqrt_dk, float* probs,
+                            long long probs_plane, cudaStream_t stream);
+/* F.cross_entropy(x, tgt, reduction="none") of espnet_model.py:57 in fp32: out[r] = logsumexp(x[r][0..V-1]) - x[r][tgt[r]] (row pitch ld),
+ * each row read once with a running max; out[r] = 0 where tgt[r] < 0 (the positions nll zeroes), NaN where tgt[r] >= V. */
+int espb_nll_rows_f32(const float* x, long long rows, long long ld, int V, const int* tgt, float* out, cudaStream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
