@@ -10,6 +10,7 @@ import torch
 import torch.nn.functional as F
 
 import rnn_fixture as fx
+import test_rnn_host as rh
 from oracle import rnn as orn
 
 pytestmark = pytest.mark.gpu
@@ -340,3 +341,343 @@ def test_bin_asr_inference_from_config_and_checkpoint(tmp_path):
         assert tok[0] == "a" and tok[1:] == [str(t) for t in hyps[k - 1][0][1:-1]]
         score = float((tmp_path / f"dec/{k}best_recog/score").read_text().split()[1])
         assert abs(score - hyps[k - 1][1]) <= TOL * abs(hyps[k - 1][1])
+
+
+# ================================================================================ kernels at recipe shapes, tile edges and refusals
+# Against the float64 references of tests/test_rnn_host.py (vgg_conv1_ref, vgg_pool_ref, lstm_step_ref, att_loc_ref), fed the values the
+# kernels read; each returns a per-element bound of the kernel's fp32 arithmetic, derived in its docstring, and err <= bound is asserted
+# everywhere.  Outputs start as NaN: what a kernel must not write keeps its NaN bits.
+NAN = float("nan")
+NAN_BITS = int(np.float32(NAN).view(np.int32))
+
+
+def _nan_bits(t):
+    return bool((t.view(torch.int32) == NAN_BITS).all())
+
+
+def _within(got, ref, tol, what):
+    err = (got - ref).abs()
+    assert bool((err <= tol).all()), f"{what}: max err {err.max().item():.3e}, worst err/tol {(err / tol.clamp_min(1e-300)).max().item():.2f}"
+
+
+def _refused(name, args, match, *untouched):
+    from espnet_b200 import ops
+
+    with pytest.raises(RuntimeError, match=match):
+        ops.call(name, *args)
+    torch.cuda.synchronize()
+    for t in untouched:
+        assert _nan_bits(t) if t.is_floating_point() else bool((t == 1).all())
+
+
+@pytest.mark.parametrize("B,Tf,T,Fr,C,lens", [(3, 3000, 3000, 83, 64, [3000, 1, 1237]), (2, 1001, 1000, 80, 96, [999, 1]),
+                                             (2, 301, 301, 80, 256, [301, 150])])
+def test_vgg_conv1_recipe_shapes(B, Tf, T, Fr, C, lens):
+    """F 83 (fbank + pitch) and 80; T up to 3000 with lengths 1 and odd ones; T < Tf_max (the feature rows past T are not read); C 96 (two
+    channel groups per 256-thread block, 64 threads idle) and C 256 (one time step per block)."""
+    from espnet_b200 import ops
+
+    g = torch.Generator().manual_seed(T + C)
+    fe = torch.randn(B, Tf, Fr, generator=g)
+    fe[:, T:] = NAN                                    # rows T..Tf_max-1 are never read
+    w, b = torch.randn(C, 9, generator=g) / 3, 0.1 * torch.randn(C, generator=g)
+    fe_d, w_d, b_d, l_d = fe.cuda(), w.cuda(), b.cuda(), torch.tensor(lens, dtype=torch.int32).cuda()
+    out = torch.full((B, 2, Fr + 2, T + 2, C), NAN, device="cuda")
+    ops.call("espb_vgg_conv1_relu_f32", ops.ptr(fe_d), B, Tf, Fr, ops.ptr(l_d), ops.ptr(w_d), ops.ptr(b_d), C, ops.ptr(out), T)
+    for i, L in enumerate(lens):
+        got = (out[i, 0].double() + out[i, 1].double())
+        v, tol = rh.vgg_conv1_ref(fe_d[i, :T].double().nan_to_num(0.0), w_d.double(), b_d.double(), L)
+        exp, et = torch.zeros_like(got), torch.zeros_like(got)
+        exp[1:-1, 1:-1], et[1:-1, 1:-1] = v.permute(2, 1, 0), tol.permute(2, 1, 0)
+        _within(got, exp, et, f"conv1 T{T} F{Fr} C{C} utt {i}")
+    del out
+    torch.cuda.empty_cache()
+
+
+@pytest.mark.parametrize("B,Fr,T,C,lens", [(4, 41, 53, 128, [53, 1, 20, 27]), (3, 83, 2999, 64, [2999, 1, 1501])])
+@pytest.mark.parametrize("pool,flat", [(1, 0), (1, 1), (0, 0)])
+def test_vgg_pool_layouts_odd_extents(B, Fr, T, C, lens, pool, flat):
+    """Pool (ceil mode over the valid rows) or copy into the bordered split layout, and pool into the flat [B * To][C * Fo] rows the BLSTM
+    reads, at C 128 with odd F and T and at the F 83 / T 2999 input extents."""
+    from espnet_b200 import ops
+
+    g = torch.Generator().manual_seed(T * 7 + pool + 2 * flat)
+    x = torch.rand(B, Fr, T, C, generator=g)
+    xd, l_d = x.cuda(), torch.tensor(lens, dtype=torch.int32).cuda()
+    Fe, Te = ((Fr + 1) // 2, (T + 1) // 2) if pool else (Fr, T)
+    if flat:
+        out = torch.full((2, B * Te, C * Fe), NAN, device="cuda")
+        plane = B * Te * C * Fe
+    else:
+        out = torch.full((B, 2, Fe + 2, Te + 2, C), NAN, device="cuda")
+        plane = (Fe + 2) * (Te + 2) * C
+    ops.call("espb_vgg_pool_f32", ops.ptr(xd), B, Fr, T, C, ops.ptr(l_d), pool, flat, ops.ptr(out), plane)
+    for i, L in enumerate(lens):
+        xi = xd[i].permute(2, 1, 0).double()                # [C][T][F]
+        if pool:
+            v, tol = rh.vgg_pool_ref(xi, L)
+        else:
+            v = xi.clone()
+            v[:, L:] = 0
+            tol = 16 * rh.U32 * v.abs()
+        if flat:
+            got = (out[0].double() + out[1].double()).view(B, Te, C * Fe)[i]
+            exp, et = v.transpose(0, 1).reshape(Te, C * Fe), tol.transpose(0, 1).reshape(Te, C * Fe)
+        else:
+            got = out[i, 0].double() + out[i, 1].double()
+            exp, et = torch.zeros_like(got), torch.zeros_like(got)
+            exp[1:-1, 1:-1], et[1:-1, 1:-1] = v.permute(2, 1, 0), tol.permute(2, 1, 0)
+        _within(got, exp, et, f"pool {pool} flat {flat} T{T} utt {i}")
+
+
+def test_vgg_refusals():
+    from espnet_b200 import ops
+
+    fe, w, b = torch.zeros(1, 8, 5, device="cuda"), torch.zeros(257 * 9, device="cuda"), torch.zeros(257, device="cuda")
+    lens = torch.tensor([8], dtype=torch.int32).cuda()
+    out = torch.full((2 * 7 * 10 * 257,), NAN, device="cuda")
+    base = dict(T=8, F=5, C=64)
+    for bad in (dict(C=0), dict(C=257), dict(T=9), dict(F=0)):
+        a = dict(base, **bad)
+        _refused("espb_vgg_conv1_relu_f32", (ops.ptr(fe), 1, 8, a["F"], ops.ptr(lens), ops.ptr(w), ops.ptr(b), a["C"], ops.ptr(out), a["T"]),
+                 "vgg_conv1_relu: need", out)
+    x = torch.zeros(5 * 8 * 64, device="cuda")
+    for bad in (dict(F=0), dict(T=0), dict(C=0), dict(C=-3), dict(F=-1)):
+        a = dict(base, **bad)
+        _refused("espb_vgg_pool_f32", (ops.ptr(x), 1, a["F"], a["T"], a["C"], ops.ptr(lens), 1, 0, ops.ptr(out), 7 * 10 * 64),
+                 "vgg_pool: need", out)
+
+
+def _lstm_lens(B, T, g):
+    return [T, T - 1, 1] + torch.randint(1, T + 1, (B - 3,), generator=g).tolist()
+
+
+@pytest.mark.parametrize("H,Hp", [(320, 320), (1024, 1024), (333, 336)])
+@pytest.mark.parametrize("ndir", [1, 2])
+def test_lstm_rec_step_recipe_widths(H, Hp, ndir):
+    """The (B)LSTM recurrence at the recipes' widths 320 and 1024 and at H 333 < Hp 336, B 16 with ragged lengths {T, T - 1, 1, ..}, gate
+    pre-activations randn and +-60 (saturated sigmoid and tanh), y rows ldy > ndir * H.  Each step against lstm_step_ref fed the gates,
+    the h W_hh^T product and the c the kernel holds; the pad columns of h (H..Hp) and of y (ndir * H..ldy) keep their NaN, and y rows
+    t >= len are +0."""
+    from espnet_b200 import ops
+
+    g = torch.Generator().manual_seed(H * ndir)
+    B, T = 16, 7
+    lens = _lstm_lens(B, T, g)
+    xg = torch.randn(B, T, ndir * 4 * H, generator=g) * 2
+    sat = torch.rand(B, T, ndir * 4 * H, generator=g) < 0.3
+    xg[sat] = 60 * torch.sign(xg[sat])
+    whh = (torch.randn(ndir, 4 * H, H, generator=g) / H ** 0.5).double().cuda()
+    ldy = ndir * H + 3
+    xgd, l32 = xg.cuda(), torch.tensor(lens, dtype=torch.int32).cuda()
+    h = torch.full((2, ndir, B, Hp), NAN, device="cuda")
+    c = torch.full((ndir, B, H), NAN, device="cuda")
+    hg = torch.zeros(ndir, B, 4 * H, device="cuda")
+    y = torch.full((2, B * T, ldy), NAN, device="cuda")
+    L = torch.tensor(lens).cuda()
+    bi = torch.arange(B, device="cuda")
+    for s in range(T):
+        if s:
+            hg.copy_(torch.einsum("dbk,dgk->dbg", _hl(h)[:, :, :H].double(), whh).float())
+        c_prev = c.double()
+        ops.call("espb_lstm_rec_step_f32", ops.ptr(xgd), ops.ptr(hg), ops.ptr(l32), s, B, T, H, Hp, ndir, ops.ptr(h), ndir * B * Hp,
+                 ops.ptr(c), ops.ptr(y), B * T * ldy, ldy)
+        yv = _hl(y.double()).view(B, T, ldy)
+        for d in range(ndir):
+            act = s < L
+            t = torch.where(act, (L - 1 - s) if d else torch.full_like(L, s), 0)
+            xs = xgd[bi, t, d * 4 * H:(d + 1) * 4 * H].double()
+            hr, cr, th, tc = rh.lstm_step_ref(xs, None if s == 0 else hg[d].double(), c_prev[d])
+            what = f"H{H} ndir{ndir} s{s} d{d}"
+            _within(_hl(h.double())[d, act, :H], hr[act], th[act], what + " h")
+            _within(c[d, act].double(), cr[act], tc[act], what + " c")
+            _within(yv[bi, t, d * H:(d + 1) * H][act], hr[act], th[act], what + " y")
+    assert _nan_bits(h[..., H:]) and _nan_bits(y[..., ndir * H:])
+    for b, n in enumerate(lens):
+        assert not bool(y[:, b * T + n:(b + 1) * T, :ndir * H].ne(0).any()), f"utterance {b}: y rows past len not 0"
+
+
+def test_lstm_rec_step_refusals():
+    from espnet_b200 import ops
+
+    H = 8
+    xg, hg = torch.zeros(2 * 4 * 2 * H, device="cuda"), torch.zeros(2 * 2 * 4 * H, device="cuda")
+    lens = torch.tensor([2], dtype=torch.int32).cuda()
+    h, c, y = (torch.full((n,), NAN, device="cuda") for n in (2 * 2 * H, 2 * H, 2 * 2 * 2 * H))
+    base = dict(s=0, H=H, Hp=H, ndir=2, ldy=2 * H)
+    for bad in (dict(Hp=H - 1), dict(ndir=3), dict(ndir=0), dict(ldy=2 * H - 1), dict(s=-1)):
+        a = dict(base, **bad)
+        _refused("espb_lstm_rec_step_f32", (ops.ptr(xg), ops.ptr(hg), ops.ptr(lens), a["s"], 1, 2, a["H"], a["Hp"], a["ndir"], ops.ptr(h),
+                                            2 * H, ops.ptr(c), ops.ptr(y), 2 * 2 * H, a["ldy"]), "lstm_rec_step: need", h, c, y)
+
+
+@pytest.mark.parametrize("act", [0, 1])
+@pytest.mark.parametrize("write_plain,with_out", [(0, True), (1, False)])
+def test_rnn_proj_post_modes(act, write_plain, with_out):
+    """write_plain = 0 with out: x bit-unchanged; out = NULL with write_plain = 1: x in place only.  D = 13 (not a multiple of 4) with
+    ldo = 16: the pad columns keep their NaN."""
+    from espnet_b200 import ops
+
+    g = torch.Generator().manual_seed(act + 2 * write_plain)
+    B, T, D, ldo = 3, 5, 13, 16
+    lens = [5, 2, 1]
+    x = torch.randn(B, T, D, generator=g)
+    xd, l_d = x.cuda(), torch.tensor(lens, dtype=torch.int32).cuda()
+    out = torch.full((2, B * T, ldo), NAN, device="cuda")
+    ops.call("espb_rnn_proj_post_f32", ops.ptr(xd), B, T, D, ops.ptr(l_d), act, write_plain, ops.ptr(out) if with_out else None,
+             B * T * ldo, ldo)
+    exp = torch.tanh(x.double()) if act else x.double()
+    for b, n in enumerate(lens):
+        exp[b, n:] = 0
+    tol = (5 * rh.U32) * exp.abs()                            # tanhf 4u and its fp32 rounding; the identity is exact
+    if write_plain:
+        _within(xd.cpu().double(), exp, tol, "x in place")
+    else:
+        assert torch.equal(xd.cpu().view(torch.int32), x.view(torch.int32))
+    if with_out:
+        _within(_hl(out.double())[:, :D].cpu().view(B, T, D), exp, tol + 16 * rh.U32 * exp.abs(), "out")
+        assert _nan_bits(out[:, :, D:])
+    else:
+        assert _nan_bits(out)
+
+
+def test_rnn_proj_post_refusal():
+    from espnet_b200 import ops
+
+    x = torch.randn(2, 3, 8, device="cuda")
+    x0 = x.clone()
+    l_d = torch.tensor([3, 1], dtype=torch.int32).cuda()
+    out = torch.full((2, 6, 8), NAN, device="cuda")
+    _refused("espb_rnn_proj_post_f32", (ops.ptr(x), 2, 3, 8, ops.ptr(l_d), 1, 1, ops.ptr(out), 48, 7), "rnn_proj_post: need ldo >= D", out)
+    assert torch.equal(x, x0)
+    ops.call("espb_rnn_proj_post_f32", ops.ptr(x), 2, 3, 8, ops.ptr(l_d), 1, 1, None, 0, 7)   # ldo is not read without out
+    torch.cuda.synchronize()
+    assert bool(x[1, 1:].eq(0).all()) and not torch.equal(x, x0)
+
+
+@pytest.mark.parametrize("j", [0, 4])
+def test_drop_cand_several_blocks(j):
+    from espnet_b200 import ops
+
+    n, PC = 600, 5
+    valid = torch.ones(n, PC, dtype=torch.int32, device="cuda")
+    ops.call("espb_drop_cand_i32", ops.ptr(valid), n, PC, j)
+    exp = torch.ones(n, PC, dtype=torch.int32)
+    exp[:, j] = 0
+    assert torch.equal(valid.cpu(), exp)
+    for bad in (-1, PC):
+        v = torch.ones(n, PC, dtype=torch.int32, device="cuda")
+        _refused("espb_drop_cand_i32", (ops.ptr(v), n, PC, bad), r"drop_cand: need 0 <= j < PC", v)
+
+
+def _att_setup(A, E, chans, filts, Tmax, lens, W, seed, peaked):
+    """Weights, encoder states (split) and device operands of AttLoc for len(lens) utterances x W slots."""
+    from espnet_b200 import ops
+
+    w, _, _, g = rh._att_case(A, E, chans, filts, 1, seed, peaked)
+    U = len(lens)
+    enc = torch.randn(U, Tmax, E, generator=g)
+    d = rh._att_dev_inputs(w, enc, torch.zeros(16))
+    enc_split = ops.split_from(enc.cuda().view(U * Tmax, E))
+    dev = {k: v.cuda() for k, v in d.items() if k != "dz"}
+    dev["lens"] = torch.tensor(lens, dtype=torch.int32).cuda()
+    return dict(w=w, g=g, enc_split=enc_split, enc_v=_hl(enc_split.double()).view(U, Tmax, E), dev=dev, U=U, W=W, n=U * W, Tmax=Tmax,
+                A=A, E=E, chans=chans, filts=filts, lens=lens)
+
+
+def _att_call(st, dz, anc, pos, step, ring, out, out_ld, out2):
+    from espnet_b200 import ops
+
+    dv, n, E = st["dev"], st["n"], st["E"]
+    ops.call("espb_att_loc_step_f32", ops.ptr(dv["eh"]), ops.ptr(st["enc_split"]), st["U"] * st["Tmax"] * E, ops.ptr(dv["lens"]), st["W"],
+             st["Tmax"], st["A"], E, ops.ptr(dz), ops.ptr(dv["cw"]), st["chans"], st["filts"], ops.ptr(dv["wt"]), ops.ptr(dv["gv"]),
+             ops.ptr(dv["gb"]), ops.ptr(anc), anc.shape[1], pos, ops.ptr(step), ops.ptr(ring), n, ops.ptr(out), n * out_ld, out_ld,
+             ops.ptr(out2), 0 if out2 is None else n * E, E)
+
+
+def _att_check(st, dz, prev_ring, anc, pos, ring, out, what):
+    """Every slot's new ring row and context against att_loc_ref, fed the parent's ring row the kernel read (1/len in fp32 at pos 0)."""
+    dv, E = st["dev"], st["E"]
+    ring_c = ring[pos & 1].double()
+    ctx = _hl(out.double())
+    for s in range(st["n"]):
+        u = s // st["W"]
+        L = st["lens"][u]
+        prev = (torch.full((L,), float(np.float32(1.0) / np.float32(L)), dtype=torch.float64, device="cuda") if pos == 0
+                else prev_ring[int(anc[s, pos - 1])][:L].double())
+        a, c, ta, tc = rh.att_loc_ref(dv["eh"][u].double(), dz[s].double(), dv["cw"].double(), dv["wt"].double(), dv["gv"].double(),
+                                      dv["gb"].double(), st["enc_v"][u], prev, L)
+        _within(ring_c[s, :L], a, ta, f"{what} pos {pos} slot {s} weights")
+        assert not bool(ring[pos & 1, s, L:].ne(0).any()), f"{what} pos {pos} slot {s}: weights past len not 0"
+        _within(ctx[s, :E], c, tc, f"{what} pos {pos} slot {s} context")
+
+
+@pytest.mark.parametrize("A,E,chans,filts,Tmax,peaked", [(1024, 1024, 10, 100, 750, False), (320, 320, 10, 100, 1500, False),
+                                                          (320, 320, 10, 100, 750, True)])
+def test_att_loc_step_recipe_shapes(A, E, chans, filts, Tmax, peaked):
+    """AttLoc at the aishell RNN recipe's adim 1024 (10 channels, 100 taps: about 76 KiB of shared memory at Tmax 750, 30 s of audio) and
+    at adim 320 with Tmax 1500 (about 70 KiB), both above the 48 KiB default, and a peaked case (gvec x 60, 2e spans hundreds).  Lengths
+    Tmax, 1, 57 (< filts) and Tmax - 1, W = 4 slots each; positions 0, 1, 2 with parents reordered through the ancestor table; out_ld = E + 5
+    (pad columns keep their NaN), out2 at position 0 only (bitwise out); position 1 again as pos 0 + *step_ptr = 1 is bitwise position 1."""
+    lens = [Tmax, 1, 57, Tmax - 1]
+    st = _att_setup(A, E, chans, filts, Tmax, lens, 4, seed=A + Tmax + peaked, peaked=peaked)
+    n, W, g = st["n"], st["W"], st["g"]
+    anc = torch.tensor([[(s // W) * W + (3 * s + 1) % W, (s // W) * W + (s + 2) % W] for s in range(n)], dtype=torch.int32).cuda()
+    ring = torch.full((2, n, Tmax), NAN, device="cuda")
+    out_ld = E + 5
+    outs = [torch.full((2, n, out_ld), NAN, device="cuda") for _ in range(3)]
+    out2 = torch.full((2, n, E), NAN, device="cuda")
+    wdec = st["w"]["att_list.0.mlp_dec.weight"].double()
+    prev_ring = None
+    what = f"A{A} Tmax{Tmax}{' peaked' if peaked else ''}"
+    for pos in range(3):
+        dz = (torch.randn(n, wdec.shape[1], generator=g, dtype=torch.float64) @ wdec.t()).float().cuda()
+        _att_call(st, dz, anc, pos, None, ring, outs[pos], out_ld, out2 if pos == 0 else None)
+        torch.cuda.synchronize()
+        if pos == 0:
+            assert _nan_bits(ring[1]), "position 0 wrote the other ring half"
+            assert torch.equal(out2, outs[0][:, :, :st["E"]])
+        _att_check(st, dz, prev_ring, anc, pos, ring, outs[pos], what)
+        assert _nan_bits(outs[pos][:, :, st["E"]:])
+        if pos == 1:
+            snap = ring[1].clone()
+            again = torch.full_like(outs[1], NAN)
+            step = torch.ones(1, dtype=torch.int32, device="cuda")
+            _att_call(st, dz, anc, 0, step, ring, again, out_ld, None)
+            torch.cuda.synchronize()
+            assert torch.equal(again.view(torch.int32), outs[1].view(torch.int32)) and torch.equal(ring[1], snap), "step_ptr"
+        prev_ring = ring[pos & 1].clone()
+
+
+def test_att_loc_step_largest_shared_memory():
+    """adim 1024, 10 channels, 100 taps: Tmax 3969 is the largest whose shared memory (4 (12 Tmax + 200 + 10240) bytes plus the 132-byte
+    reduction buffer) fits the 227 KiB a block may use; it runs and is right.  Tmax 3970 is refused before any launch."""
+    st = _att_setup(1024, 64, 10, 100, 3969, [3969, 1], 1, seed=3, peaked=False)
+    wdec = st["w"]["att_list.0.mlp_dec.weight"].double()
+    dz = (torch.randn(2, wdec.shape[1], generator=st["g"], dtype=torch.float64) @ wdec.t()).float().cuda()
+    anc = torch.zeros(2, 1, dtype=torch.int32, device="cuda")
+    ring = torch.full((2, 2, 3969), NAN, device="cuda")
+    out = torch.full((2, 2, 64), NAN, device="cuda")
+    _att_call(st, dz, anc, 0, None, ring, out, 64, None)
+    torch.cuda.synchronize()
+    _att_check(st, dz, None, anc, 0, ring, out, "Tmax 3969")
+
+
+@pytest.mark.parametrize("bad,match", [(dict(Tmax=3970), "too large for shared memory"), (dict(Tmax=5000), "too large for shared memory"),
+                                       (dict(W=5), "W > 0 dividing n"), (dict(out_ld=63), "out_ld"), (dict(filts=-1), "filts >= 0")])
+def test_att_loc_step_refusals(bad, match):
+    """Each bad argument is refused with a message before any launch: ring and out keep their NaN."""
+    from espnet_b200 import ops
+
+    a = dict(A=1024, E=64, chans=10, filts=100, Tmax=64, W=4, out_ld=64)
+    a.update(bad)
+    n = 12
+    f = lambda k: torch.zeros(k, device="cuda")   # noqa: E731
+    eh, enc, dz, cw, wt, gv, gb = f(3 * a["Tmax"] * a["A"]), f(2 * 3 * a["Tmax"] * 64), f(n * a["A"]), f(10 * 201), f(10 * a["A"]), f(a["A"]), f(1)
+    lens = torch.full((3,), 5, dtype=torch.int32, device="cuda")
+    anc = torch.zeros(n, 2, dtype=torch.int32, device="cuda")
+    ring = torch.full((2, n, a["Tmax"]), NAN, device="cuda")
+    out = torch.full((2, n, 64), NAN, device="cuda")
+    _refused("espb_att_loc_step_f32", (ops.ptr(eh), ops.ptr(enc), 3 * a["Tmax"] * 64, ops.ptr(lens), a["W"], a["Tmax"], a["A"], a["E"],
+                                       ops.ptr(dz), ops.ptr(cw), a["chans"], a["filts"], ops.ptr(wt), ops.ptr(gv), ops.ptr(gb), ops.ptr(anc), 2,
+                                       0, None, ops.ptr(ring), n, ops.ptr(out), n * 64, a["out_ld"], None, 0, 64), match, ring, out)

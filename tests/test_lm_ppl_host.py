@@ -3,6 +3,7 @@ checkpoints, the sos / eos / padding logic of nll and the full-sequence forwards
 the files calc_perplexity writes, and the refusals.  Against tests/golden/lm_ppl.npz (make_golden_lm_ppl.py, the UNMODIFIED reference)."""
 import ctypes
 import json
+import math
 import os
 
 import numpy as np
@@ -151,3 +152,138 @@ def test_capi_entry_points_bound():
         handle = ctypes.CDLL(lib.LIB_PATH)
         for name in ("espb_causal_flash_attn_f32", "espb_causal_softmax_f32", "espb_nll_rows_f32"):
             assert hasattr(handle, name)
+
+
+# ------------------------------------------------------------------------------------------------ float64 references of the kernels
+# The values the kernels read in, the result and a per-element bound of the kernel's fp32 arithmetic out (u = 2^-24; expf within 2 ulp
+# <= 4u, logf 1 ulp; a value stored split as hi + lo is within 16u).  tests/test_gpu_lm_ppl.py asserts err <= bound;
+# test_tolerances_catch_plausible_bugs below shows each bound is tight enough to see the bugs named there.  Peaked scores give key weights
+# below fp32's smallest normal 2^-126 (__expf flushes them to 0): the bounds add 2^-126 absolute per weight.
+U32 = 2.0 ** -24
+TINY = 2.0 ** -126
+
+
+def _over(diff, tol):
+    return (diff / tol.clamp_min(1e-300)).max().item()
+
+
+def _valid_keys(tok, n, T, diag=0, mask_tok=True, device=None):
+    i, j = torch.arange(T, device=device).view(T, 1), torch.arange(T, device=device).view(1, T)
+    ok = (j <= i + diag) & (j < n)
+    return ok & (tok != 0).view(1, T) if mask_tok else ok
+
+
+def causal_attn_ref(q, k, v, tok, lens, scale=0.125, diag=0, mask_tok=True):
+    """Causal token-masked attention (espb_causal_flash_attn_f32) of q / k / v [B][H][T][64] float64, tok [B][T], lens -> (o, tol), rows
+    without a valid key 0.  diag / mask_tok / scale restate bugs: keys up to i + diag admitted, token-0 keys not masked, another scale.
+    The bound is the one derived for the fused kernel in tests/test_gpu_attention.py (3xTF32 scores within 67u sum_c |q_c k_c|, a key
+    weight off relatively by rho = e_s scale + 4u (m - s scale) + (4 nkt + 20) u, P V in 3xTF32, the row sum and 1 / l) with the counts of
+    the causal kernel: a row i of the 128-row block starting at I0 runs nkt = ceil(min(len, I0 + 128) / 64) key tiles, and each thread sums
+    a quarter of those keys."""
+    B, H, T, _ = q.shape
+    o, tol = torch.zeros_like(q), torch.zeros_like(q)
+    i0 = torch.arange(T, device=q.device) // 128 * 128
+    for b, n in enumerate(lens):
+        n = min(int(n), T)
+        if n <= 0:
+            continue
+        ok = _valid_keys(tok[b].to(q.device), n, T, diag, mask_tok, q.device)
+        nk = (i0 + 128).clamp(max=n).double().view(T, 1)
+        nkt = torch.ceil(nk / 64)
+        s = q[b] @ k[b].transpose(-1, -2)
+        es = 67 * U32 * (q[b].abs() @ k[b].abs().transpose(-1, -2))
+        z = torch.where(ok, s * scale, torch.full((), -math.inf, dtype=q.dtype, device=q.device))
+        m = z.max(-1, keepdim=True).values
+        has = torch.isfinite(m)
+        p = torch.where(ok, torch.exp(z - torch.where(has, m, torch.zeros_like(m))), torch.zeros((), dtype=q.dtype, device=q.device))
+        p = p / p.sum(-1, keepdim=True).clamp_min(1e-300)
+        ob = p @ v[b]
+        rho = torch.where(ok, es * scale + 4 * U32 * (torch.where(has, m, torch.zeros_like(m)) - z).abs(), torch.zeros_like(z)) \
+            + (4 * nkt + 20) * U32
+        pr = p * rho
+        va = v[b].abs()
+        tol[b] = pr @ va + pr.sum(-1, keepdim=True) * ob.abs() + (66 + nkt) * U32 * (p @ va) + (nk / 4 + nkt + 20) * U32 * ob.abs() \
+            + TINY * (1 + va.sum(-2, keepdim=True))
+        o[b] = ob
+    return o, tol
+
+
+def causal_softmax_ref(sc, tok, lens, sqrt_dk, Tp):
+    """espb_causal_softmax_f32 of scores sc [B][H][T][Tp] float64 -> (probs, tol) [B][H][T][Tp], pitch columns and rows without a valid key 0.
+    Per key: a = s / sqrt_dk and x = a - max round once each (u |a|, u |x|), expf 4u; each lane sums ceil(nk / 32) terms, 5 shuffle adds;
+    the divide u; the split store 16u.  rho_j = u (|a_j| + |x_j| + 4) + sum_k p_k u (|a_k| + |x_k| + 4) + (ceil(nk / 32) + 22) u."""
+    B, H, T, _ = sc.shape
+    pr, tol = torch.zeros_like(sc), torch.zeros_like(sc)
+    for b, n in enumerate(lens):
+        ok = torch.zeros(T, Tp, dtype=torch.bool, device=sc.device)
+        ok[:, :T] = _valid_keys(tok[b].to(sc.device), min(int(n), T), T, device=sc.device)
+        a = sc[b] / sqrt_dk
+        z = torch.where(ok, a, torch.full((), -math.inf, dtype=sc.dtype, device=sc.device))
+        m = z.max(-1, keepdim=True).values
+        m = torch.where(torch.isfinite(m), m, torch.zeros_like(m))
+        p = torch.where(ok, torch.exp(z - m), torch.zeros((), dtype=sc.dtype, device=sc.device))
+        p = p / p.sum(-1, keepdim=True).clamp_min(1e-300)
+        e = torch.where(ok, U32 * (a.abs() + (a - m).abs() + 4), torch.zeros_like(a))
+        nk = torch.arange(T, device=sc.device).clamp(max=int(n) - 1).double().view(T, 1) + 1
+        rho = e + (p * e).sum(-1, keepdim=True) + (torch.ceil(nk / 32) + 22) * U32
+        pr[b], tol[b] = p, torch.where(ok, p * rho + TINY, torch.zeros_like(p))
+    return pr, tol
+
+
+def nll_ref(x, tgt, ncols=None):
+    """espb_nll_rows_f32 of logits x [R][V] float64 (the first ncols columns only: a bug) -> (out, tol); 0 where tgt < 0, NaN where
+    tgt >= V.  With m the row max and p_j the softmax: each thread's running logsumexp takes its terms with expf (4u) of an argument
+    rounded by u |x_j - m| and adds them in sequence (n = ceil(V / 256) + 3 terms per thread at most, float4 or scalar loads), rescaling
+    its sum at most n times by expf of a rounded difference whose magnitudes add up to at most the row's spread r = m - min x (and so do
+    those of the 12 merges across lanes and warps, each two expf and two roundings); then logf (2u |log s|), x_t - m (u) and the final
+    subtraction (u):  tol = u (sum_j p_j (4 + |x_j - m|) + 6 n + 72 + 2 r + 2 |log s| + |x_t - m| + |out|)."""
+    R, V = x.shape
+    xs = x if ncols is None else x[:, :ncols]
+    t = tgt.long()
+    lse = torch.logsumexp(xs, -1)
+    xt = x.gather(1, t.clamp(0, V - 1).view(R, 1)).view(R)
+    out = lse - xt
+    m = x.max(-1).values
+    p = torch.softmax(x, -1)
+    n = -(-V // 256) + 3
+    ls = (lse - m).abs()
+    tol = U32 * ((p * (4 + (x - m.view(R, 1)).abs())).sum(-1) + 6 * n + 72 + 2 * (m - x.min(-1).values) + 2 * ls + (xt - m).abs()
+                 + out.abs())
+    out = torch.where(t < 0, torch.zeros_like(out), torch.where(t >= V, torch.full_like(out, math.nan), out))
+    return out, tol
+
+
+def _attn_case(B, H, T, lens, seed, qscale=1.0, device="cpu"):
+    """Seeded q / k / v [B][H][T][64] and token ids: token 0 at every 7th key from 3, at keys 64 and 128, and in the last sentence at every
+    key before min(T - 1, 97) when B > 1 (the rows before have no valid key, row 97's only valid key is its own)."""
+    g = torch.Generator().manual_seed(seed)
+    q, k, v = (torch.randn(B, H, T, 64, generator=g, dtype=torch.float64) * 0.5 for _ in range(3))
+    q = q * qscale
+    tok = torch.randint(1, 9, (B, T), generator=g, dtype=torch.int32)
+    tok[:, 3::7] = 0
+    tok[:, 64:65] = 0
+    tok[:, 128:129] = 0
+    if B > 1 and T > 1:
+        tok[-1, :min(T - 1, 97)] = 0
+    return q.to(device), k.to(device), v.to(device), tok
+
+
+def test_tolerances_catch_plausible_bugs():
+    """On the CPU, from the float64 references above: each plausible bug moves the reference by more than 10x the tolerance the GPU tests
+    of tests/test_gpu_lm_ppl.py use, at a shape they run: in the causal attention (B 2, T 193) one key past the diagonal admitted, the
+    token-0 mask ignored and 1 / d_k in place of 1 / sqrt(d_k); in the NLL (V 257, the row maximum in the last column) a logsumexp over
+    V - 1 columns."""
+    B, H, T, lens = 2, 1, 193, [193, 193]
+    q, k, v, tok = _attn_case(B, H, T, lens, seed=T)
+    ref, tol = causal_attn_ref(q, k, v, tok, lens)
+    assert float(tol.max()) < 1e-4
+    for bug in (dict(diag=1), dict(mask_tok=False), dict(scale=1.0 / 64)):
+        o, _ = causal_attn_ref(q, k, v, tok, lens, **bug)
+        assert _over((o - ref).abs(), tol) > 10, bug
+    g = torch.Generator().manual_seed(257)
+    x = (torch.rand(6, 257, generator=g, dtype=torch.float64) * 2 - 1) * 80
+    x[0, -1] = 80
+    tgt = torch.tensor([256, 3, 7, 100, 0, 200], dtype=torch.int32)
+    out, tl = nll_ref(x, tgt)
+    out2, _ = nll_ref(x, tgt, ncols=256)
+    assert float(tl.max()) < 1e-4 and _over((out2 - out).abs(), tl) > 10

@@ -7,6 +7,7 @@ import re
 import numpy as np
 import pytest
 import torch
+import torch.nn.functional as F
 
 import rnn_fixture as fx
 from oracle import rnn as orn
@@ -196,3 +197,184 @@ def test_decoder_host_logic_vs_oracle(context_residual, monkeypatch):
                 torch.testing.assert_close(st["c"][pos & 1, k, s, :H].double(), ns[1][k], atol=2e-5, rtol=0)
             torch.testing.assert_close(st["a"][pos & 1, s, :Lu].double(), ns[2], atol=2e-5, rtol=0)
         prev = cur
+
+
+# ------------------------------------------------------------------------------------------------ float64 references of the kernels
+# Each takes the values the kernel reads (fp32 inputs as float64, hi + lo of split operands) and returns the result with a per-element error
+# bound of the kernel's fp32 arithmetic, u = 2^-24.  CUDA's expf and tanhf are within 2 ulp (<= 4u relative), logf within 1 ulp, and a value
+# stored split (hi + lo, each with 10 explicit mantissa bits) is within 2^-20 = 16u of the fp32 result.  tests/test_gpu_rnn.py compares the
+# kernels with these; test_tolerances_catch_plausible_bugs below shows the bounds are tight enough to see the bugs named there.  Saturated
+# gates and peaked weights reach values below fp32's smallest normal 2^-126, which keep no relative precision: the bounds add 2^-126
+# absolute where that happens.
+U32 = 2.0 ** -24
+TINY = 2.0 ** -126
+
+
+def _over(diff, tol):
+    """max diff / tol (diff > 0 where tol == 0 counts as infinitely over)."""
+    return (diff / tol.clamp_min(1e-300)).max().item()
+
+
+def vgg_conv1_ref(x, w, b, L):
+    """conv1_1 + ReLU (espb_vgg_conv1_relu_f32) of one utterance x [T][F] with rows t >= L zero, w [C][9], b [C] -> (v, tol) [C][T][F].
+    Per element 9 fmaf and the bias add, each within u of the partial sums' magnitude sum_k |w_k x_k| + |b|, then the split store."""
+    C = w.shape[0]
+    x = x.clone()
+    x[L:] = 0
+    v = torch.relu(F.conv2d(x[None, None], w.view(C, 1, 3, 3), b, padding=1))[0]
+    mag = F.conv2d(x.abs()[None, None], w.abs().view(C, 1, 3, 3), b.abs(), padding=1)[0]
+    v[:, L:] = 0
+    return v, 10 * U32 * mag + 16 * U32 * v.abs()
+
+
+def vgg_pool_ref(x, L, ceil=True):
+    """2x2 max-pool of x [C][T][F] over its rows t < L (espb_vgg_pool_f32, ceil mode) -> (v [C][To][Fo], tol): the max is exact, so the
+    tolerance is the split store.  ceil=False restates a pool in floor mode (odd T or F lose their last row or column)."""
+    C, T, Fr = x.shape
+    To, Fo = (T + 1) // 2, (Fr + 1) // 2
+    r = F.max_pool2d(x[None, :, :L], 2, stride=2, ceil_mode=ceil)[0]
+    v = x.new_zeros(C, To, Fo)
+    v[:, :r.shape[1], :r.shape[2]] = r
+    return v, 16 * U32 * v.abs()
+
+
+def _sig(x):
+    s = torch.sigmoid(x)
+    return s, s * (1 - s)
+
+
+def lstm_step_ref(xg, hg, cp, order=(0, 1, 2, 3)):
+    """One LSTM cell step (espb_lstm_rec_step_f32): gates xg [..][4H] (+ hg, None at the first step, where c starts at 0), c_prev cp
+    [..][H] as the kernel holds it -> (h, c, tol_h, tol_c).  order restates a gate layout bug ((1, 0, 2, 3): i and f swapped).
+    Error per element: the gate sum xg + hg rounds once (u |x|, moved by sigma' = s (1 - s) or tanh' = 1 - tanh^2); sigmoid
+    1 / (1 + expf(-x)) is within 6u relative (expf, the add, the divide), tanhf within 4u; c' = s_f c + s_i tanh(g) rounds twice; h' =
+    s_o tanhf(c') once more; h (and y) are stored split (16u), c plain."""
+    x = xg if hg is None else xg + hg
+    dx = torch.zeros_like(x) if hg is None else U32 * x.abs()
+    gi, gf, gg, go = (x.chunk(4, dim=-1)[k] for k in order)
+    di, df, dg, do = (dx.chunk(4, dim=-1)[k] for k in order)
+    cp = torch.zeros_like(gi) if hg is None else cp
+    (si, si_d), (sf, sf_d), (so, so_d) = _sig(gi), _sig(gf), _sig(go)
+    tg = torch.tanh(gg)
+    e_si, e_sf, e_so = 6 * U32 * si + si_d * di, 6 * U32 * sf + sf_d * df, 6 * U32 * so + so_d * do
+    e_tg = 4 * U32 * tg.abs() + (1 - tg * tg) * dg
+    c = sf * cp + si * tg
+    e_c = e_sf * cp.abs() + e_si * tg.abs() + si * e_tg + 2 * U32 * ((sf * cp).abs() + (si * tg).abs())
+    tc = torch.tanh(c)
+    h = so * tc
+    e_h = e_so * tc.abs() + so * (4 * U32 * tc.abs() + (1 - tc * tc) * e_c) + 17 * U32 * h.abs() + 4 * TINY
+    return h, c, e_h, e_c + 4 * TINY
+
+
+def att_loc_ref(eh, dz, cw, wt, gv, gb, enc, prev, L, tap=0, len_off=0):
+    """AttLoc of one slot (espb_att_loc_step_f32) from the values the kernel reads: eh [>= L][A] = mlp_enc(enc) + bias, dz [A] = mlp_dec(z),
+    cw [chans][2 filts + 1], wt [chans][A] (mlp_att.weight^T), gv [A], gb, enc [>= L][E] (hi + lo), prev [L] the previous weights (the
+    uniform 1/L of the first step as the fp32 value the kernel forms) -> (a [L], ctx [E], tol_a, tol_ctx).  OracleRNNDecoder.att
+    (oracle/rnn.py) computes the same from the model weights; test_att_loc_ref_is_the_oracle checks that.
+    tap / len_off restate bugs: the location conv reads prev one tap late; the softmax runs over L + len_off frames.
+    Error, per frame t: the conv (K = 2 filts + 1 fmaf) within K u sum_k |w prev|; loc = sum_c wt conv (chans fmaf) within chans u
+    sum_c |wt conv| plus the conv errors through |wt|; the two adds into the tanh argument u (|loc| + |eh| + |dz|) each; tanhf 4u; the energy
+    (ceil(A / 32) fmaf per lane, 5 shuffle adds, + gb) within (ceil(A / 32) + 6) u (sum_a |gv tanh| + |gb|), doubled by the scaling 2.
+    A weight a_t = exp(x_t - m) / sum is off relatively by its own energy error and the weighted mean of all of them (through the sum),
+    u |x_t - m| for the subtraction, 4u for expf (in its own term and, weighted, in the sum's), and (ceil(L / 256) + 12) u for the block sum (per-thread adds, two 5-step shuffle
+    trees), 1 / sum and the product.  The context
+    (hi + lo added, then L fmaf in sequence) is within sum_t tol_a |enc| + (L + 1) u sum_t a |enc|, plus 16u for its split store.  Weights
+    whose exponential underflows (peaked energies) are within 2^-126."""
+    K, A = cw.shape[1], wt.shape[1]
+    filts = (K - 1) // 2
+    Lw = L + len_off
+    pv = prev.new_zeros(Lw)
+    pv[:min(L, Lw)] = prev[:min(L, Lw)]
+    pp = F.pad(pv, (filts - tap, filts + tap))[None, None]
+    conv = F.conv1d(pp, cw[:, None])[0].t()                              # [Lw][chans]
+    e_conv = K * U32 * F.conv1d(pp.abs(), cw.abs()[:, None])[0].t()
+    loc = conv @ wt
+    e_loc = wt.shape[0] * U32 * (conv.abs() @ wt.abs()) + e_conv @ wt.abs()
+    arg = loc + eh[:Lw] + dz
+    e_arg = e_loc + 2 * U32 * (loc.abs() + eh[:Lw].abs() + dz.abs())
+    th = torch.tanh(arg)
+    e_th = 4 * U32 * th.abs() + (1 - th * th) * e_arg
+    x = 2 * (th @ gv + gb)
+    e_x = 2 * (e_th @ gv.abs() + (-(-A // 32) + 6) * U32 * (th.abs() @ gv.abs() + abs(float(gb))))
+    a = torch.softmax(x, 0)
+    xm = (x - x.max()).abs()
+    rho = e_x + (a * e_x).sum() + U32 * (xm + (a * xm).sum()) + (20 - (-Lw // 256)) * U32
+    ta = a * rho + TINY
+    en = enc[:Lw]
+    ctx = a @ en
+    tc = ta @ en.abs() + (Lw + 1) * U32 * (a @ en.abs()) + 16 * U32 * ctx.abs() + TINY
+    return a, ctx, ta, tc
+
+
+def _att_case(A, E, chans, filts, Tmax, seed, peaked=False):
+    """Seeded weights and inputs of one AttLoc slot at the given shape, and its OracleRNNDecoder; gvec scaled by 60 when peaked (2e spans
+    hundreds)."""
+    g = torch.Generator().manual_seed(seed)
+    H = 16
+    w = {"att_list.0.mlp_enc.weight": torch.randn(A, E, generator=g) / E ** 0.5, "att_list.0.mlp_enc.bias": 0.1 * torch.randn(A, generator=g),
+         "att_list.0.mlp_dec.weight": torch.randn(A, H, generator=g) / H ** 0.5, "att_list.0.mlp_att.weight": torch.randn(A, chans, generator=g),
+         "att_list.0.loc_conv.weight": torch.randn(chans, 1, 1, 2 * filts + 1, generator=g) / 4,
+         "att_list.0.gvec.weight": torch.randn(1, A, generator=g) / A ** 0.5 * (60 if peaked else 1),
+         "att_list.0.gvec.bias": 0.1 * torch.randn(1, generator=g)}
+    enc = torch.randn(Tmax, E, generator=g)
+    z = torch.randn(H, generator=g)
+    return w, enc, z, g
+
+
+def _att_dev_inputs(w, enc, z):
+    """The values the attention kernel reads, from the model weights: eh, dz rounded to fp32 as the GEMMs deliver them (float64 here)."""
+    eh = (enc.double() @ w["att_list.0.mlp_enc.weight"].double().t() + w["att_list.0.mlp_enc.bias"].double()).float()
+    dz = (w["att_list.0.mlp_dec.weight"].double() @ z.double()).float()
+    chans = w["att_list.0.mlp_att.weight"].shape[1]
+    return dict(eh=eh, dz=dz, cw=w["att_list.0.loc_conv.weight"].view(chans, -1).contiguous(), wt=w["att_list.0.mlp_att.weight"].t().contiguous(),
+                gv=w["att_list.0.gvec.weight"].view(-1).contiguous(), gb=w["att_list.0.gvec.bias"].contiguous())
+
+
+def test_att_loc_ref_is_the_oracle():
+    """att_loc_ref over mlp_enc(enc) and mlp_dec(z) in float64 is OracleRNNDecoder.att, first step and a later one."""
+    w, enc, z, g = _att_case(40, 24, 3, 5, 30, seed=1)
+    o = orn.OracleRNNDecoder(orn.to(w), 1)
+    x = {k: v.double() for k, v in dict(eh=enc.double() @ w["att_list.0.mlp_enc.weight"].double().t() + w["att_list.0.mlp_enc.bias"].double(),
+                                        dz=w["att_list.0.mlp_dec.weight"].double() @ z.double()).items()}
+    d = {k: v.double() for k, v in _att_dev_inputs(w, enc, z).items()}
+    L = 23
+    for prev in (None, torch.softmax(torch.randn(L, generator=g, dtype=torch.float64), 0)):
+        c_o, a_o = o.att(enc[:L].double(), z.double(), prev)
+        p = torch.full((L,), 1.0 / L, dtype=torch.float64) if prev is None else prev
+        a, c, _, _ = att_loc_ref(x["eh"], x["dz"], d["cw"], d["wt"], d["gv"], d["gb"], enc.double(), p, L)
+        torch.testing.assert_close(a, a_o, atol=1e-12, rtol=0)
+        torch.testing.assert_close(c, c_o, atol=1e-12, rtol=0)
+
+
+def test_tolerances_catch_plausible_bugs():
+    """On the CPU, from the float64 references above: each plausible bug moves the reference by more than 10x the tolerance the GPU tests
+    of tests/test_gpu_rnn.py use, at a shape they run.
+    * LSTM i and f gates swapped (H 320, B 16, gates randn and +-60);
+    * the location conv one tap late, and the softmax over len + 1 frames (AttLoc at adim 1024, 10 channels, 100 taps, Tmax 750, len 57,
+      previous weights of a later step);
+    * the pool in floor mode (C 128, odd F 41 and T 53)."""
+    g = torch.Generator().manual_seed(0)
+    H = 320
+    xg = torch.randn(16, 4 * H, generator=g, dtype=torch.float64) * 2
+    xg[:, ::3] = 60 * torch.sign(xg[:, ::3])
+    hg = torch.randn(16, 4 * H, generator=g).double()
+    cp = torch.randn(16, H, generator=g).double()
+    h, c, th, tcl = lstm_step_ref(xg, hg, cp)
+    h2, c2, _, _ = lstm_step_ref(xg, hg, cp, order=(1, 0, 2, 3))
+    assert float(th.max()) < 1e-5 and _over((h2 - h).abs(), th) > 10 and _over((c2 - c).abs(), tcl) > 10
+
+    A, E, chans, filts, Tmax, L = 1024, 1024, 10, 100, 750, 57
+    w, enc, z, g = _att_case(A, E, chans, filts, Tmax, seed=2)
+    d = {k: v.double() for k, v in _att_dev_inputs(w, enc, z).items()}
+    prev = torch.softmax(3 * torch.randn(L, generator=g, dtype=torch.float64), 0).float().double()
+    args = (d["eh"], d["dz"], d["cw"], d["wt"], d["gv"], d["gb"], enc.double(), prev, L)
+    a, ctx, ta, tc = att_loc_ref(*args)
+    for bug in (dict(tap=1), dict(len_off=1)):
+        a2, ctx2, _, _ = att_loc_ref(*args, **bug)
+        assert _over((a2[:L] - a).abs(), ta) > 10, bug
+        assert _over((ctx2 - ctx).abs(), tc) > 10, bug
+
+    x = torch.rand(128, 53, 41, generator=g, dtype=torch.float64)
+    v, tol = vgg_pool_ref(x, 53)
+    v2, _ = vgg_pool_ref(x, 53, ceil=False)
+    assert _over((v2 - v).abs(), tol) > 10
